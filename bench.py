@@ -38,31 +38,6 @@ sys.path.insert(0, ROOT)
 GPT4 = r"""'(?i:[sdmt]|ll|ve|re)|[^\r\n\p{L}\p{N}]?+\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]++[\r\n]*|\s*[\r\n]|\s+(?!\S)|\s+"""
 
 
-def kernel_source_sha():
-    """sha256 over the sources of the dominant kernel (k_merge_seg): a committed ncu capture is only quoted
-    while it describes the kernel that is being timed."""
-    import hashlib
-    h = hashlib.sha256()
-    for f in ("k_merge_seg.cuh", "k_merge.cuh", "common.cuh", "k_seg.cuh"):
-        h.update(open(os.path.join(ROOT, "minbpe_b200", "csrc", f), "rb").read())
-    return h.hexdigest()[:16]
-
-
-def ncu_traffic():
-    """DRAM bytes of one profiled launch of the dominant kernel (ncu --set full, committed under profiles/);
-    null when no capture of the CURRENT kernel source is on record (the capture carries the source hash)."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        d = json.load(open(p))
-    except Exception:  # noqa: BLE001
-        return None, None
-    sha = kernel_source_sha()
-    if d.get("kernel_source_sha") != sha:
-        return None, {"stale": True, "capture_sha": d.get("kernel_source_sha"), "current_sha": sha,
-                      "note": "profiles/ncu_traffic.json was captured from another version of the kernel; re-run tools/ncu_traffic.sh"}
-    return d["dram_bytes"], d
-
-
 from minbpe_b200.presplit import host_cores  # noqa: E402  (affinity mask capped by the cgroup CPU quota)
 
 
@@ -73,7 +48,24 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s at up to 700 W; not a measured peak)"
+
+
+def gpu_identity(gpu=0):
+    """Name and power limit of the GPU the line was measured on: a time or a rate means nothing without them."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                              "-i", str(gpu)], capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception:  # noqa: BLE001
+        return None
+
+
+def dump_outputs(directory, arrays):
+    """--dump-outputs: the arrays the timed call returned, as float64 .npy files (ids and counts are exact in float64)."""
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), np.asarray(a, dtype=np.float64))
 
 
 # Test hook: tests/test_emu.py runs this file end to end (all legs, N = 1 and 2 ranks over gloo, tiny sizes) against the
@@ -922,7 +914,7 @@ def run_sharded(args, rank, world, local):
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     eng = E.Engine(local)
     eng.set_option(E.OPT_KERNEL_TIMING, 1)
-    eng.set_option(E.OPT_HIST_KERNEL, 2)      # iteration-0 histogram with the kernel that has run on B200s (see run_ours)
+    eng.set_option(E.OPT_HIST_KERNEL, 2)      # iteration-0 histogram with the library's default kernel (see run_ours)
     step = make_step_engine(eng, local)
     sampler = None
     if rank == 0:
@@ -998,10 +990,11 @@ def run_sharded(args, rank, world, local):
                        "parallelism": f"shard{world}", "prep_s": round(prep_s, 1), "consistent": bool(ok),
                        "exchange_used": tr.exchange, "exchange_fallback_reason": getattr(tr, "exchange_fallback", None),
                        "shard_bytes_rank0": int(hi - lo),
-                       "l2": "per-GPU stream >> 126 MB L2, re-read from HBM every step",
+                       "l2": "per-GPU stream >> 50 MB L2, re-read from HBM every step",
                        "timing": "CUDA events on the shared stream, max over ranks, barrier + synchronize on both sides"},
             "merges_per_s": K / t, "wall_ms_per_step": wall / K * 1e3,
             "gpu_launches": int(tm["kernel_launches"]),
+            "gpu": None if EMU else gpu_identity(local),
             "clocks": clocks,
             "phases_ms": {"step": k_ms, "merge_kernels_per_rank": [float(x.item()) for x in merge_all],
                           "select_exchange_apply": k_ms - max(float(x.item()) for x in merge_all),
@@ -1022,6 +1015,8 @@ def run_sharded(args, rank, world, local):
                     "what": "per rank: bpe_load_text_gpt4(host shard text: H2D + device split) + sharded loop of W+K merges + merges D2H, wall clock, max over ranks"},
             "first_pairs": pairs[W:W + 4].tolist(), "merges_sha16": merges_sha(pairs[: W + K]),
         }
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"merges": pairs[W:W + K], "counts": counts[W:W + K]})
     # ---- optional detail legs (every rank arms the same watchdog: a leg that hangs ends all ranks, rank 0 printing the
     #      contract line as it stands; a leg that raises on every rank is reported as {"error": ...}) ----
     dog = Watchdog(args.leg_budget_s)
@@ -1089,8 +1084,8 @@ def run_ours(args):
         torch.cuda.set_device(local)
     eng = E.Engine(local)
     eng.set_option(E.OPT_KERNEL_TIMING, 1)
-    # the contract line is measured on kernels that have run on B200s: the iteration-0 histogram with k_hist_dense (the
-    # library's default); the automatic choice (cross-check + timing of k_hist_dense_packed) is the `hist_packed` leg below
+    # the iteration-0 histogram with k_hist_dense (the library's default); the automatic choice (cross-check + timing of
+    # k_hist_dense_packed) is the `hist_packed` leg below
     eng.set_option(E.OPT_HIST_KERNEL, 2)
 
     sampler = ClockSampler(local)
@@ -1130,6 +1125,8 @@ def run_ours(args):
     tm = eng.timing()
     assert done == K
     assert np.array_equal(pairs, pairs_e2e[W:W + K]), "timed run and e2e run disagree"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"merges": pairs, "counts": counts})
     t_loop = tm["loop_ms"] / 1e3          # CUDA events on the library's stream, around the K iterations
     value = size * K / t_loop / 1e9
     n_in, n_out = tm["tokens_in"], tm["tokens_out"]
@@ -1142,7 +1139,7 @@ def run_ours(args):
         "dtype": "int32", "data": "synthetic",
         "config": {"workload": f"BASELINE configs[2]: RegexTokenizer.train merge loop (GPT-4 split) on {args.size_mib} MiB synthetic "
                                f"UTF-8 seed {args.seed}, merge steps {W}..{W + K - 1} of 32512", "tokens_start": int(raw.size),
-                   "chunks": prep["chunks"], "l2": "stream (>= 4 bytes/token, far larger than the 126 MB L2) is re-read from HBM every step",
+                   "chunks": prep["chunks"], "l2": "stream (>= 4 bytes/token, far larger than the 50 MB L2) is re-read from HBM every step",
                    "timing": "CUDA events on the library stream around the K enqueued iterations; wall-clock check in wall_ms_per_step",
                    "prep": prep},
         "merges_per_s": K / t_loop,
@@ -1150,10 +1147,10 @@ def run_ours(args):
         "algorithmic_GBps_survey_8d": (8.0 * n_in + 4.0 * n_out) / t_loop / 1e9,
         "wall_ms_per_step": wall / K * 1e3,
         "gpu_launches": int(tm["kernel_launches"]),
+        "gpu": None if EMU else gpu_identity(local),
         "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": "k_merge_seg (fused merge + in-place segment compaction + stats delta)",
-                     "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": ncu_traffic()[0],
-                     "traffic_capture": ncu_traffic()[1],
+                     "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                      "peak_source": peak_src, "bytes_per_launch": (4.0 * n_in + 4.0 * n_out) / K, "ms_per_launch": k_ms,
                      "loop_frac_in_kernel": tm["merge_kernel_ms"] / tm["loop_ms"]},
         "cpu_baseline": cpu,
@@ -1198,7 +1195,7 @@ def run_ours(args):
 
 
 def run_extras(args):
-    """--extras: side measurements recorded in profiles/ (not the contract line): cfg2 wall times and
+    """--extras: side measurements (not the contract line): cfg2 wall times and
     chunk-parallel encode throughput (BASELINE configs[1] and configs[4] shapes)."""
     import torch
     from minbpe_b200 import BasicTokenizer, RegexTokenizer
@@ -1270,9 +1267,11 @@ def main():
     ap.add_argument("--full-merges", type=int, default=32512,
                     help="N=1: also run the whole train() loop (this many merges, configs[2] = 32512) from the host text "
                          "and compare every merge with the oracle; 0 = skip")
-    ap.add_argument("--strong-gib", type=int, default=16,
+    ap.add_argument("--strong-gib", type=int, default=4,
                     help="also run BASELINE configs[3] (strong scaling: this many GiB in total over the N GPUs, vocab "
-                         "--strong-vocab) and report it as strong_cfg4; 0 = skip")
+                         "--strong-vocab) and report it as strong_cfg4; 0 = skip.  A GPU holds 8 bytes per corpus byte of its "
+                         "shard (two 4-byte token buffers) plus the split working set of one piece, so one 80 GB H100 takes "
+                         "4 GiB with room to spare; 16 GiB needs 4 or more")
     ap.add_argument("--strong-mib", type=int, default=0, help="size of the strong leg in MiB instead of --strong-gib (small runs, tests)")
     ap.add_argument("--strong-vocab", type=int, default=100000)
     ap.add_argument("--strong-sparse-at", type=int, default=1000, help="first merge of the second (sparse) timed window of the strong leg")
@@ -1283,8 +1282,8 @@ def main():
     ap.add_argument("--encode-merges", type=int, default=32512, help="merges of the table the encode leg uses when the run has not trained one")
     ap.add_argument("--encode-train-mib", type=int, default=256, help="... trained on this many MiB of the cfg3 corpus")
     ap.add_argument("--exchange", default=os.environ.get("BPE_EXCHANGE", "collective"), choices=["collective", "p2p"],
-                    help="N>1: per-merge exchange of the sharded loop. collective = two NCCL all-reduces (validated on 2/4/8 B200s); "
-                         "p2p = the hand-written NVLink peer-memory kernels of k_xchg.cuh (opt-in until validated on hardware)")
+                    help="N>1: per-merge exchange of the sharded loop. collective = two NCCL all-reduces; "
+                         "p2p = the hand-written NVLink peer-memory kernels of k_xchg.cuh (opt-in)")
     ap.add_argument("--leg-budget-s", type=int, default=600,
                     help="wall-clock budget of the optional legs (whole-loop run, cfg4, cfg5) after the contract line is complete; "
                          "when it runs out the line is printed with the legs finished so far")
@@ -1293,6 +1292,9 @@ def main():
     ap.add_argument("--no-p2p-trial", action="store_true", help="N>1: skip the trial of the NVLink peer-memory exchange kernels")
     ap.add_argument("--no-filter-leg", action="store_true", help="skip the full_run_filtered leg (N=1)")
     ap.add_argument("--extras", action="store_true", help="side measurements (cfg2 wall time, encode throughput)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what they returned (merges [K,2] and counts [K] of the K timed merges; "
+                         "rank 0 for N>1) as DIR/<name>.npy in float64, to compare two builds output for output")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

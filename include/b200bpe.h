@@ -1,5 +1,5 @@
 /*
- * b200bpe.h — C ABI of libb200bpe.so, the B200 (sm_100a) BPE train/encode hot path.
+ * b200bpe.h — C ABI of libb200bpe.so, the H100 (sm_90a) BPE train/encode hot path.
  *
  * The reference (karpathy/minbpe @1acefe8) is pure Python and has no FFI; its hot path is
  * the three primitives in minbpe/base.py plus the loops in basic.py / regex.py that drive
@@ -43,7 +43,7 @@ typedef enum {
 /* ---- lifetime ------------------------------------------------------------------------ */
 
 /* Create a handle bound to CUDA device `device`.  Fails with BPE_ERR_CUDA when there is no
- * usable sm_100 device: there is NO CPU fallback.  (Stands where the reference constructs a
+ * usable sm_90 device: there is NO CPU fallback.  (Stands where the reference constructs a
  * Tokenizer, base.py:69-74 — the handle is the device-side state of one tokenizer.) */
 int bpe_create(int device, bpe_handle **out);
 int bpe_destroy(bpe_handle *h);
@@ -264,7 +264,7 @@ int bpe_get_timing(bpe_handle *h, bpe_timing *out);
                                    a piece are cut where a letter is followed by U+0020 (process-wide) */
 #define BPE_OPT_SPLIT_PATTERN 8 /* which of the reference's two split patterns (regex.py:18-19) the *_gpt4 entry points apply:
                                    0 = GPT4_SPLIT_PATTERN (default), 1 = GPT2_SPLIT_PATTERN; per handle */
-#define BPE_OPT_HIST_KERNEL 9   /* byte-pair histogram of iteration 0: 2 = k_hist_dense (default: the kernel that has run on B200s);
+#define BPE_OPT_HIST_KERNEL 9   /* byte-pair histogram of iteration 0: 2 = k_hist_dense (default);
                                    1 = k_hist_dense_packed; 0 = k_hist_dense until the first stream of >= 8 Mi tokens, where
                                    k_hist_dense_packed is cross-checked and timed against it and adopted if equal and not slower */
 #define BPE_OPT_SEG_FILTER 10   /* bpe_train: skip the segments a merge cannot touch (per-segment id signatures + candidate list,

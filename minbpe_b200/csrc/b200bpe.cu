@@ -1,7 +1,7 @@
-// b200bpe.cu — host side of libb200bpe.so: the C ABI of include/b200bpe.h over the sm_100a
+// b200bpe.cu — host side of libb200bpe.so: the C ABI of include/b200bpe.h over the sm_90a
 // kernels in k_load.cuh / k_stats.cuh / k_merge.cuh / k_encode.cuh.
 //
-// Build: see build.py (nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -shared).
+// Build: see build.py (nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -shared).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -82,7 +82,7 @@ struct bpe_handle {
     int opt_memo_log2 = 0;   // BPE_OPT_ENC_MEMO_LOG2 (test hook): log2 slots of the encode memo table, 0 = default
     u32 opt_vocab_cap = 0;   // BPE_OPT_VOCAB_CAP: lower bound of the delta-vector layout V used by bpe_train
     int opt_seg_filter = 0;      // BPE_OPT_SEG_FILTER: 0 = off, 1 = switch it on when merges have become sparse, 2 = always
-    int opt_hist_kernel = 2;     // BPE_OPT_HIST_KERNEL: 2 = k_hist_dense (default: the kernel that has run on B200s), 1 = k_hist_dense_packed,
+    int opt_hist_kernel = 2;     // BPE_OPT_HIST_KERNEL: 2 = k_hist_dense (default), 1 = k_hist_dense_packed,
                                  // 0 = decide at the first large stream (cross-check + timing)
     int opt_split_pattern = 0;   // BPE_OPT_SPLIT_PATTERN: 0 = GPT-4 split pattern, 1 = GPT-2 (bpe_split_gpt4 / bpe_load_text_gpt4 / bpe_encode_text_gpt4*)
 
@@ -157,10 +157,10 @@ extern "C" int bpe_create(int device, bpe_handle **out) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) return fail(nullptr, BPE_ERR_CUDA, cudaGetErrorString(e));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
         return fail(nullptr, BPE_ERR_CUDA, std::string("bpe_create: device '") + prop.name + "' is sm_" +
                                                std::to_string(prop.major) + std::to_string(prop.minor) +
-                                               "; this library contains sm_100a code only");
+                                               "; this library contains sm_90a code only");
     h = new (std::nothrow) bpe_handle();
     if (!h) return fail(nullptr, BPE_ERR_INTERNAL, "out of host memory");
     h->device = device;
@@ -612,7 +612,7 @@ static int ensure_delta(bpe_handle *h, u32 V) {
 // emulator, so a handle's first histogram of a LARGE stream (>= 8 Mi tokens; smaller ones just take k_hist_dense) runs both
 // kernels, timed with events, and compares all 65,536 counters on the device: equal and not slower -> the packed kernel
 // from then on; otherwise (or 128 KB of shared memory refused) -> k_hist_dense stays.  bpe_timing.hist_kernel
-// reports which one is in use.  (Drop the cross-check once `pytest -m gpu` has passed on a B200 with hist_kernel == 1.)
+// reports which one is in use.  (Drop the cross-check once `pytest -m gpu` has passed with hist_kernel == 1 on every GPU model in use.)
 #define HIST_DECIDE_MIN_TOKENS (8ull << 20)   /* smaller streams say nothing about speed: they take k_hist_dense, undecided */
 static int hist_dense(bpe_handle *h, ull *dense_out) {
     const int grid_old = h->sms * 3;

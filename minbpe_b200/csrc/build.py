@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """Builds the in-tree native libraries of minbpe_b200 (no network, no JIT cache):
 
-  libb200bpe.so    hand-written sm_100a kernels + the C ABI of include/b200bpe.h   (nvcc)
-  libbpesynth.so   synthetic corpus generator for bench/tests                       (gcc)
+  libb200bpe.so    hand-written sm_90a (H100) kernels + the C ABI of include/b200bpe.h   (nvcc)
+  libbpesynth.so   synthetic corpus generator for bench/tests                             (gcc)
 
 nvcc cross-compiles without a GPU.  Called by __graft_entry__.build().
 """
@@ -12,7 +12,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-CUDA_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+CUDA_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
 

@@ -1,4 +1,4 @@
-// common.cuh — shared definitions for the sm_100a BPE kernels.
+// common.cuh — shared definitions for the sm_90a BPE kernels.
 #pragma once
 #ifndef BPE_SIMT_EMU
 #include <cuda_runtime.h>
@@ -163,7 +163,7 @@ __device__ __forceinline__ u32 ld_volatile_u32(const u32 *p) {
 __device__ __forceinline__ u32 lane_id() { return threadIdx.x & 31; }
 
 #ifndef BPE_SIMT_EMU
-// ---- mbarrier + bulk async copy (TMA 1-D) — hand-written PTX for sm_100a ---------------------
+// ---- mbarrier + bulk async copy (TMA 1-D) — hand-written PTX for sm_90a ----------------------
 __device__ __forceinline__ u32 smem_addr(const void *p) { return (u32)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(u64 *bar, u32 count) {

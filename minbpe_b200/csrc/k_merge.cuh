@@ -36,10 +36,9 @@ __device__ __forceinline__ u32 desc_status(u64 d) { return (u32)(d >> 36) & 3u; 
 __device__ __forceinline__ u64 desc_value(u64 d) { return d & 0xfffffffffull; }
 
 // Decoupled look-back, executed by one full warp.  Returns the exclusive prefix of `agg`.
-// NOTE (profiles/r1_lookback.md): with ~450 tiles in flight the chain of inclusive prefixes is
-// the critical path of a contiguous compaction on B200 (the known-prefix frontier moves one
-// 32-tile window per L2 round trip, ~1.3-1.5 TB/s of stream traffic); the segmented stream of
-// k_merge_seg.cuh exists to avoid it.  This contiguous kernel remains for pairs (a,a) and packing.
+// NOTE: with hundreds of tiles in flight the chain of inclusive prefixes is the critical path
+// of a contiguous compaction (the known-prefix frontier moves one 32-tile window per L2 round
+// trip); the segmented stream of k_merge_seg.cuh exists to avoid it.  This contiguous kernel remains for pairs (a,a) and packing.
 __device__ __forceinline__ u64 tile_lookback(u64 *desc, u32 tile, u32 epoch, u64 agg) {
     const u32 lane = lane_id();
     if (tile == 0) {

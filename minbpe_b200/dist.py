@@ -175,9 +175,9 @@ class ShardedTrainer:
     rank's shard (Engine.load_stream)."""
 
     def __init__(self, eng, rank=None, world=None, group=None, poll_every=16, exchange=None):
-        """exchange: "collective" = two torch.distributed all-reduces per merge (NCCL / gloo) — the default: it is the
-        path that has been validated on 2/4/8 B200s; "p2p" = our kernels over NVLink peer memory (k_xchg.cuh), opt-in
-        (argument, or BPE_EXCHANGE=p2p) until it has run on multi-GPU hardware (DESIGN.md §5)."""
+        """exchange: "collective" = two torch.distributed all-reduces per merge (NCCL / gloo) — the default;
+        "p2p" = our kernels over NVLink peer memory (k_xchg.cuh), opt-in (argument, or BPE_EXCHANGE=p2p) until it has run on
+        multi-GPU hardware (DESIGN.md §5)."""
         self.eng, self.group = eng, group
         self.rank = dist.get_rank(group) if rank is None else rank
         self.world = dist.get_world_size(group) if world is None else world

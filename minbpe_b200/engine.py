@@ -1,7 +1,7 @@
 """
 ctypes binding of libb200bpe.so (include/b200bpe.h) — the only door between the Python host
-classes and the sm_100a kernels.  There is NO CPU fallback: if the library is missing or no
-B200 is present, every operation raises.
+classes and the sm_90a kernels.  There is NO CPU fallback: if the library is missing or no
+H100 is present, every operation raises.
 """
 import ctypes
 import os

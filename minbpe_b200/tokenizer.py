@@ -15,7 +15,7 @@ short texts (third-party ``regex`` module, regex.py:41,114), special-token split
 (regex.py:123-164), vocab construction and the save/load file format (base.py:88-165), decode
 (basic.py:51-55, regex.py:78-90).
 
-There is no CPU fallback: without libb200bpe.so and a B200 the device-backed calls raise.
+There is no CPU fallback: without libb200bpe.so and an H100 the device-backed calls raise.
 """
 import unicodedata
 

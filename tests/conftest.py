@@ -4,8 +4,8 @@ import sys
 
 import pytest
 
-# The GPU tests run the byte-pair histogram of iteration 0 with k_hist_dense, the kernel that has run on B200s (also the
-# library's default); tests/test_gpu_zz_hist.py — last group — selects the packed kernel and the automatic choice explicitly.
+# The GPU tests run the byte-pair histogram of iteration 0 with k_hist_dense, the library's default; tests/test_gpu_zz_hist.py
+# — last group — selects the packed kernel and the automatic choice explicitly.
 os.environ.setdefault("BPE_HIST_KERNEL", "2")
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -15,7 +15,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu")
 
 
 def pytest_sessionstart(session):
@@ -31,7 +31,7 @@ def pytest_sessionstart(session):
 
 
 # GPU tests that cannot be traced on the emulator (they need torch CUDA tensors): classified by hand.  1 = reaches a kernel
-# that has not run on a B200 yet (k_xchg_*), 0 = kernels that have.
+# outside the hardware-validated set (k_xchg_*), 0 = kernels inside it.
 _MANUAL_GPU_ORDER = {"test_step_api_world1[p2p]": 1, "test_step_api_world1[collective]": 0,
                      "test_step_api_world2_nccl[p2p]": 1, "test_step_api_world2_nccl[collective]": 0,
                      # left out of the coverage run for their size; both launch the split / training kernels only
@@ -39,9 +39,9 @@ _MANUAL_GPU_ORDER = {"test_step_api_world1[p2p]": 1, "test_step_api_world1[colle
 
 
 def pytest_collection_modifyitems(config, items):
-    """The driver runs `pytest -x -m gpu`: order the GPU tests so that tests launching only kernels that have already run on
-    a B200 come first and tests reaching a kernel known only to the CPU emulator come last (map: tests/emu/kernel_coverage.json,
-    written by tests/emu/kernel_coverage.py).  A kernel that misbehaves on real hardware then costs the tests behind it, not
+    """For `pytest -x -m gpu`: order the GPU tests so that tests launching only kernels of the hardware-validated set come
+    first and tests reaching any other kernel come last (map and set: tests/emu/kernel_coverage.json, written by
+    tests/emu/kernel_coverage.py).  A kernel that misbehaves on real hardware then costs the tests behind it, not
     the ones that would have passed.  Order inside each group is unchanged; CPU tests are not touched."""
     path = os.path.join(ROOT, "tests", "emu", "kernel_coverage.json")
     if not os.path.exists(path):

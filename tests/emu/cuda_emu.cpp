@@ -432,7 +432,7 @@ cudaError_t cudaGetDeviceCount(int *n) { *n = env_int("EMU_DEVICES", 8); return 
 cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
     memset(p, 0, sizeof(*p));
     snprintf(p->name, sizeof(p->name), "SIMT emulator (CPU, tests/emu)");
-    p->major = 10; p->minor = 0;
+    p->major = 9; p->minor = 0;
     p->multiProcessorCount = env_int("EMU_SMS", 2);
     return cudaSuccess;
 }

@@ -1,6 +1,6 @@
 // tests/emu/cuda_emu.h — TEST INFRASTRUCTURE: a CPU SIMT emulator for the kernel SOURCES of minbpe_b200/csrc.
 //
-// Why: the kernels can only be validated on a B200.  When no GPU is reachable (this container has none) the next best
+// Why: the kernels can only be validated on an H100.  When no GPU is reachable (a build host without one) the next best
 // check is to run the very same kernel source — same index arithmetic, same shared-memory protocol, same warp
 // collectives, same atomics, same host-side launch sequence — on the CPU and compare the C ABI's results with the
 // oracle.  tests/emu/build_emu.py rewrites only the launch syntax (`k<<<g, b, s, st>>>(args)`) and the
@@ -184,7 +184,7 @@ static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess
 cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t a, cudaEvent_t b);
 template <class F> static inline cudaError_t cudaFuncSetAttribute(F f, cudaFuncAttribute a, int v) {
     if (a == cudaFuncAttributeMaxDynamicSharedMemorySize) {
-        if (v > 227 * 1024) return cudaErrorInvalidValue;      // sm_100: 227 KB per CTA
+        if (v > 227 * 1024) return cudaErrorInvalidValue;      // sm_90: 227 KB per CTA
         emu::set_max_dyn_smem(reinterpret_cast<const void *>(f), v);
     }
     return cudaSuccess;

@@ -1,7 +1,7 @@
 """GPU: the packed dense byte-pair histogram (k_hist_dense_packed, b200bpe.cu hist_dense).  Forced on
 (BPE_OPT_HIST_KERNEL = 1) it must train exactly like the oracle; with BPE_OPT_HIST_KERNEL = 0 the library decides at the
 first large stream — both kernels run, the 65,536 counters are compared on the device and the launches timed — and
-whatever it decides, results do not change.  (Default: 2, the kernel that has run on B200s.)"""
+whatever it decides, results do not change.  (Default: 2, k_hist_dense.)"""
 import numpy as np
 import pytest
 
