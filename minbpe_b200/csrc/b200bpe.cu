@@ -56,6 +56,8 @@ struct bpe_handle {
     Edge *edge[2] = {nullptr, nullptr}; u64 *seg_offs = nullptr; u64 seg_cap = 0;  // segmented stream metadata
     ull *delta = nullptr; u32 V = 0;   // V = layout of the delta vector the kernels index (L[0,V) R[V,2V) ZZ[2V])
     u32 delta_cap = 0;                 // vocabulary capacity of the OWNED buffer `delta` (step mode uses the caller's)
+    u32 delta_vecs = 0;                // delta vectors of 2*delta_cap+1 counters in it: one per member of a batched pass
+    bool batching = false;             // bpe_train's loop may carry several merges per pass (k_select_batch)
     u32 max_id = 255;                  // largest id in the loaded stream (bpe_load_ids); byte streams: 255
     ull *dense = nullptr;
     ull *dense2 = nullptr; u32 *d_cmp = nullptr;   // first-use cross-check of the packed histogram kernel (hist_dense)
@@ -67,6 +69,7 @@ struct bpe_handle {
     u32 *d_err = nullptr;
     int *log_pairs = nullptr; long long *log_counts = nullptr; int log_cap = 0;
     Best *partials = nullptr;
+    TopList *top_partials = nullptr;   // k_select_batch: one list per block
     unsigned char *d_cls = nullptr, *d_contr = nullptr;   // code-point class / contraction tables of the GPT-4 splitter
     // sharded loop over NVLink peer memory (k_xchg.cuh): the rank's exchange block and its peers' mappings
     unsigned char *xchg = nullptr; u64 xchg_bytes = 0, xchg_stride = 0; u32 xchg_V = 0;
@@ -190,6 +193,7 @@ extern "C" int bpe_create(int device, bpe_handle **out) {
     h->argmax_grid = h->sms * 2;
     h->ff_grid = h->sms * 4;
     if ((e = cudaMalloc(&h->partials, sizeof(Best) * h->argmax_grid)) != cudaSuccess) return bail("cudaMalloc partials", e);
+    if ((e = cudaMalloc(&h->top_partials, sizeof(TopList) * h->argmax_grid)) != cudaSuccess) return bail("cudaMalloc top_partials", e);
     memset(h->h_ctl, 0, sizeof(Ctl));
     h->h_ctl->epoch = 1;
     h->h_ctl->found_pos = POS_NONE;
@@ -218,6 +222,7 @@ extern "C" int bpe_destroy(bpe_handle *h) {
     if (h->log_pairs) cudaFree(h->log_pairs);
     if (h->log_counts) cudaFree(h->log_counts);
     if (h->partials) cudaFree(h->partials);
+    if (h->top_partials) cudaFree(h->top_partials);
     if (h->d_cls) cudaFree(h->d_cls);
     if (h->d_contr) cudaFree(h->d_contr);
     if (h->d_present) cudaFree(h->d_present);
@@ -534,12 +539,13 @@ extern "C" int bpe_get_stats(bpe_handle *h, int32_t *pairs, int64_t *counts, uin
 // (which also refills every segment).  Every kernel gates itself on the device-resident pair, so
 // the whole sequence is enqueued unconditionally; `same` >= 0 lets the host skip the no-ops when
 // it knows the pair (single-step API).
-static void launch_merge(bpe_handle *h, ull *delta, int force, int same = -1, bool use_xchg = false) {
+// `batched`: the pass applies the members k_select_batch chose (bpe_train's loop only; a pair (a,a) is never batched).
+static void launch_merge(bpe_handle *h, ull *delta, int force, int same = -1, bool use_xchg = false, bool batched = false) {
     const unsigned char *xbase = use_xchg ? h->xchg : nullptr;
     if (same != 1) {
         SegArgs S;
         S.ctl = h->ctl; S.buf0 = h->buf[0]; S.buf1 = h->buf[1]; S.e0 = h->edge[0]; S.e1 = h->edge[1];
-        S.delta = delta; S.V = h->V; S.force = force; S.xbase = xbase; S.xstride = h->xchg_stride;
+        S.delta = delta; S.V = h->V; S.force = force; S.batched = batched; S.xbase = xbase; S.xstride = h->xchg_stride;
         if (h->filt_active) k_merge_seg<true><<<h->merge_grid_seg, MS_THREADS, MS_SMEM_BYTES, h->stream>>>(S);
         else k_merge_seg<false><<<h->merge_grid_seg, MS_THREADS, MS_SMEM_BYTES, h->stream>>>(S);
         h->tm.kernel_launches += 1;
@@ -591,20 +597,26 @@ static u64 auto_table_cap(bpe_handle *h, u64 n_unbounded_inserts) {
 }
 #define TABLE_MAX_LOAD 0.6
 
-// The owned delta vector must cover vocabulary capacity V; h->V (the layout every kernel indexes with) is
-// set to exactly V.  The capacity of the owned buffer is tracked separately: the step API points the
-// kernels at a caller's buffer and changes h->V without touching h->delta.
-static int ensure_delta(bpe_handle *h, u32 V) {
-    if (!h->delta || h->delta_cap < V) {
+// The owned delta vectors (`vecs` of them, one per member of a batched pass) must cover vocabulary capacity V; h->V
+// (the layout every kernel indexes with) is set to exactly V.  The capacity of the owned buffer is tracked separately:
+// the step API points the kernels at a caller's buffer and changes h->V without touching h->delta.
+static int ensure_delta(bpe_handle *h, u32 V, u32 vecs = 1) {
+    bool fresh = false;
+    if (!h->delta || h->delta_cap < V || h->delta_vecs < vecs) {
         if (h->delta) cudaFree(h->delta);
-        h->delta = nullptr; h->delta_cap = 0;
-        CU(cudaMalloc(&h->delta, (2ull * V + 1) * 8));
-        h->delta_cap = V;
+        h->delta = nullptr; h->delta_cap = 0; h->delta_vecs = 0;
+        CU(cudaMalloc(&h->delta, (u64)vecs * (2ull * V + 1) * 8));
+        h->delta_cap = V; h->delta_vecs = vecs;
+        fresh = true;
     }
-    if (h->V != V) CU(cudaMemsetAsync(h->delta, 0, (2ull * h->delta_cap + 1) * 8, h->stream));   // layout changes: all zero again
+    if (fresh || h->V != V)   // new buffer or the layout changes: all zero again
+        CU(cudaMemsetAsync(h->delta, 0, (u64)h->delta_vecs * (2ull * h->delta_cap + 1) * 8, h->stream));
     h->V = V;
     return BPE_OK;
 }
+// Batched passes index BATCH_MAX delta vectors with one 32-bit flat index (the merge kernel's shared-memory cache keys,
+// 0xffffffff = empty) and allocate them all: vocabularies up to 2^21 ids.
+static bool batch_fits(u32 V) { return V <= (1u << 21); }
 
 // Byte-pair histogram of the current (byte) stream into dense_out[65536] (zeroed by the caller).
 // k_hist_dense_packed (dense 16-bit counters in 128 KB of shared memory) replaces k_hist_dense (hashed per-block table +
@@ -719,29 +731,35 @@ static void drain_kernel_events(bpe_handle *h) {
     h->ev_used = 0;
 }
 
-static void timed_merge(bpe_handle *h, ull *delta, bool use_xchg = false) {
-    if (!h->opt_kernel_timing) { launch_merge(h, delta, 0, -1, use_xchg); return; }
+static void timed_merge(bpe_handle *h, ull *delta, bool use_xchg = false, bool batched = false) {
+    if (!h->opt_kernel_timing) { launch_merge(h, delta, 0, -1, use_xchg, batched); return; }
     while ((int)h->ev_pool.size() < h->ev_used + 2) { cudaEvent_t e; cudaEventCreate(&e); h->ev_pool.push_back(e); }
     cudaEventRecord(h->ev_pool[h->ev_used], h->stream);
-    launch_merge(h, delta, 0, -1, use_xchg);
+    launch_merge(h, delta, 0, -1, use_xchg, batched);
     cudaEventRecord(h->ev_pool[h->ev_used + 1], h->stream);
     h->ev_used += 2;
 }
 
-// ctl->overflow was raised by k_apply_delta: some delta entries of the last performed merge are
-// still pending.  Double the table (dead pairs are dropped on the way), re-run the apply.
-static int handle_overflow(bpe_handle *h) {
+// ctl->overflow was raised by k_apply_delta: some delta entries of the last performed pass are
+// still pending.  Double the table (dead pairs are dropped on the way), re-run the apply.  A batched
+// pass (nk members) re-runs every member's apply in member order: a member whose apply overflowed
+// stopped the ones after it, and re-applying a finished member changes nothing (its delta is zero).
+static int handle_overflow(bpe_handle *h, u32 nk = 1) {
     int rc;
-    while (h->h_ctl->overflow) {
-        const u64 new_cap = (h->table.mask + 1) * 2;
-        if ((rc = rehash_table(h, new_cap))) return rc;
-        if ((rc = pull_ctl(h))) return rc;
-        h->h_ctl->overflow = 0;
-        h->h_ctl->table_limit = (u64)(TABLE_MAX_LOAD * (double)new_cap);
-        if ((rc = push_ctl(h))) return rc;
-        k_apply_delta<<<(h->V + 255) / 256, 256, 0, h->stream>>>(h->table, h->ctl, h->delta, h->V, 0, 0, 0, 1, 1);
-        h->tm.kernel_launches++;
-        if ((rc = pull_ctl(h))) return rc;
+    for (u32 j = 0; j < nk; ++j) {
+        do {
+            if (h->h_ctl->overflow) {
+                const u64 new_cap = (h->table.mask + 1) * 2;
+                if ((rc = rehash_table(h, new_cap))) return rc;
+                if ((rc = pull_ctl(h))) return rc;
+                h->h_ctl->overflow = 0;
+                h->h_ctl->table_limit = (u64)(TABLE_MAX_LOAD * (double)new_cap);
+                if ((rc = push_ctl(h))) return rc;
+            }
+            k_apply_delta<<<(h->V + 255) / 256, 256, 0, h->stream>>>(h->table, h->ctl, h->delta, h->V, 0, 0, 0, 1, 1, (int)j);
+            h->tm.kernel_launches++;
+            if ((rc = pull_ctl(h))) return rc;
+        } while (h->h_ctl->overflow);
     }
     return BPE_OK;
 }
@@ -802,15 +820,23 @@ static void enqueue_iteration(bpe_handle *h) {
     k_argmax<<<h->argmax_grid, 256, 0, h->stream>>>(h->table, h->ctl, h->partials, h->log_pairs, h->log_counts);
     k_find_first<<<h->ff_grid, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->edge[0], h->edge[1], h->table, h->ctl, h->log_pairs, h->log_counts, 0);
     h->tm.kernel_launches += 2;
+    // several provably determined merges in one pass; not with the rescan mode (no delta) or the segment filter (its
+    // candidate list is the one pair's)
+    const bool batched = h->batching && !h->opt_rescan && !h->filt_active;
+    if (batched) {
+        k_select_batch<<<h->argmax_grid, 256, 0, h->stream>>>(h->table, h->ctl, h->top_partials, h->log_pairs, h->log_counts);
+        h->tm.kernel_launches++;
+    }
     if (h->filt_active) {    // candidate segments of the selected pair; k_merge_seg<true> works through that list only
         k_seg_filter<<<h->sms * 8, 256, 0, h->stream>>>(h->ctl, h->edge[0], h->edge[1], h->edge[0], h->edge[1], h->sig, h->cand);
         h->tm.kernel_launches++;
     }
     if (h->opt_rescan) timed_merge(h, nullptr);
     else {
-        timed_merge(h, h->delta);
-        k_apply_delta<<<(h->V + 255) / 256, 256, 0, h->stream>>>(h->table, h->ctl, h->delta, h->V, 0, 0, 0, 1, 0);
-        h->tm.kernel_launches++;
+        timed_merge(h, h->delta, false, batched);
+        for (int j = 0; j < (batched ? BATCH_MAX : 1); ++j)   // member order: each apply may need the pairs the one before inserted
+            k_apply_delta<<<(h->V + 255) / 256, 256, 0, h->stream>>>(h->table, h->ctl, h->delta, h->V, 0, 0, 0, 1, 0, j);
+        h->tm.kernel_launches += batched ? BATCH_MAX : 1;
     }
     if (h->filt_active) {    // the listed segments may have changed: their signatures from their tokens again
         k_sig_rebuild_cand<<<h->sms * 4, 256, 0, h->stream>>>(h->ctl, h->buf[0], h->buf[1], h->edge[0], h->edge[1], h->sig, h->cand);
@@ -835,7 +861,8 @@ extern "C" int bpe_train(bpe_handle *h, int32_t num_merges, int32_t first_idx, i
     // stream (bpe_load_ids accepts any id < 2^31-1) as well as the ids this call creates
     if ((u64)h->max_id + 1 >= 0x7fffffffull / 2) return fail(h, BPE_ERR_ARG, "bpe_train: ids of the loaded stream are too large for the dense delta vector");
     const u32 V = std::max(std::max((u32)first_idx + (u32)num_merges, h->max_id + 1), h->opt_vocab_cap);
-    if ((rc = ensure_delta(h, V))) return rc;
+    h->batching = !h->opt_rescan && batch_fits(V);
+    if ((rc = ensure_delta(h, V, h->batching ? BATCH_MAX : 1))) return rc;
     if (h->log_cap < num_merges) {
         if (h->log_pairs) cudaFree(h->log_pairs);
         if (h->log_counts) cudaFree(h->log_counts);
@@ -893,7 +920,7 @@ extern "C" int bpe_train(bpe_handle *h, int32_t num_merges, int32_t first_idx, i
         }
         if (h->h_ctl->overflow) {
             if (h->opt_rescan) return fail(h, BPE_ERR_CAPACITY, "rescan mode: pair table too small (set BPE_OPT_TABLE_LOG2)");
-            if ((rc = handle_overflow(h))) return rc;
+            if ((rc = handle_overflow(h, h->h_ctl->nk))) return rc;
         }
         done_iters = (int)h->h_ctl->iter;
         exhausted = h->h_ctl->done != 0;

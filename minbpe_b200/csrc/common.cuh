@@ -64,6 +64,10 @@ __device__ __forceinline__ u64 table_find(const Table &t, u64 key) {
 }
 
 // ---- device-resident control block ---------------------------------------------------------
+// Most merges one pass of bpe_train's loop may carry (k_select_batch): each member adds a delta vector of 2V+1 counters.
+#ifndef BATCH_MAX
+#define BATCH_MAX 4
+#endif
 // Everything the per-iteration kernels need to chain without the host: stream length, which
 // ping-pong buffer is current, the pair selected for the next merge, tickets.
 struct Ctl {
@@ -100,6 +104,9 @@ struct Ctl {
     u64 cand_ptr;     // device address of u32 cand[]
     u64 cand_sum;     // sum of n_cand over the filtered merges of this bpe_train call (statistics)
     u64 seg_sum;      // sum of nseg over the same merges
+    // batched merge pass (k_select_batch, DESIGN.md "Batched merges") — appended as well
+    u32 nk;                   // merges of the pass in flight: member 0 = (a, b) -> z, member j = (bat_a[j], bat_b[j]) -> z + j
+    int bat_a[BATCH_MAX], bat_b[BATCH_MAX];   // [0] unused
 };
 
 // ---- segmented stream ------------------------------------------------------------------------

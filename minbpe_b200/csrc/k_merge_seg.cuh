@@ -13,6 +13,10 @@
 // Work distribution: a ticket (one atomic) hands a warp MS_BATCH consecutive segments; the warp
 // loads their edge records once, then keeps MS_STAGES-1 bulk copies in flight ahead of the segment
 // it is working on.  The marking and delta rules are the ones documented in k_merge.cuh.
+//
+// Batched pass (bpe_train's loop, SegArgs.batched, ctl->nk > 1): up to BATCH_MAX token-disjoint pairs that
+// k_select_batch proved to be the next merges are marked and compacted in the same single pass, with one delta
+// vector per member (DESIGN.md "Batched merges").
 #pragma once
 #include "common.cuh"
 #include "k_merge.cuh"
@@ -40,7 +44,7 @@
 #define MS_BE (MS_BATCH + 2)                // edge records of a batch and of the segment on either side
 #define MS_DCACHE (1 << MS_DCACHE_LOG2)     // slots of the per-CTA delta cache (shared memory)
 #define MS_WARP_WORDS (MS_STAGES * MS_SW + MS_STAGES * MS_META + MS_BE * 8)
-#define MS_SMEM_BYTES (MS_WARPS * MS_WARP_WORDS * 4 + MS_WARPS * MS_STAGES * 8 + MS_DCACHE * 8 + 16)
+#define MS_SMEM_BYTES (MS_WARPS * MS_WARP_WORDS * 4 + MS_WARPS * MS_STAGES * 8 + MS_DCACHE * 8 + 16 + BATCH_MAX * 8)
 #define MS_INVALID 0xffffffffu
 static_assert(SEG_TOKENS == 512, "k_merge_seg: a lane owns 4 rows x 4 tokens of a 512-token segment");
 static_assert((MS_SW * 4) % 16 == 0 && (MS_WARP_WORDS * 4) % 16 == 0, "bulk-copy destinations must stay 16-byte aligned");
@@ -74,30 +78,67 @@ __device__ __noinline__ void delta_one(u32 at, u32 a, u32 b, u32 V, u32 *s_dkey,
         delta_cache_add(s_dkey, s_dcnt, delta, m_p2 ? 2u * V : V + tp2);
 }
 
+// ---- batched pass (ctl->nk > 1 members, k_select_batch): the members' pairs are in shared memory at mem_a,
+//      {a_j, b_j} at byte 8j.  Their ids are all distinct, so a token is the left token of at most one member. ----
+// the member whose left id is `tok` (nk: none)
+__device__ __forceinline__ u32 batch_member(u32 tok, u32 nk, u32 mem_a) {
+    u32 j = 0;
+#pragma unroll 1
+    for (; j < nk; ++j) if (lds32(mem_a + 8 * j) == (tok & TOK_MASK)) break;
+    return j;
+}
+// the member that starts at the token pair (t, nx) (nk: none)
+__device__ __forceinline__ u32 batch_start(u32 t, u32 nx, u32 nk, u32 mem_a) {
+    const u32 j = batch_member(t, nk, mem_a);
+    return (j < nk && lds32(mem_a + 8 * j + 4) == nx) ? j : nk;
+}
+
+// statistics delta of the merge of member j that starts at shared address `at`.  Member j is applied to the stream as
+// the members before it have left it: a neighbour that starts a merge of an earlier member m is z+m by then, one that
+// starts a merge of a later member is still itself.  Delta vector of member j: [j(2V+1), (j+1)(2V+1)), laid out as for
+// one merge.
+__device__ __noinline__ void delta_batch(u32 at, u32 nk, u32 mem_a, u32 z, u32 V, u32 *s_dkey, u32 *s_dcnt, ull *delta) {
+    const u32 t0 = lds32(at), tm1 = lds32o<-4>(at), tm2 = lds32o<-8>(at), tp2 = lds32o<8>(at), tp3 = lds32o<12>(at);
+    const u32 j = batch_member(t0, nk, mem_a);
+    const u32 ml = batch_start(tm2, tm1, nk, mem_a);   // member starting two tokens earlier
+    const u32 mr = batch_start(tp2, tp3, nk, mem_a);   // member starting two tokens later
+    const u32 base = j * (2u * V + 1u);
+    if (tm1 != TOK_SENTINEL && !(t0 & TOK_FLAG) && ml != j)
+        delta_cache_add(s_dkey, s_dcnt, delta, base + (ml < j ? z + ml : tm1 & TOK_MASK));
+    if (!(tp2 & TOK_FLAG))
+        delta_cache_add(s_dkey, s_dcnt, delta, base + (mr == j ? 2u * V : V + (mr < j ? z + mr : tp2)));
+}
+
 struct SegArgs {
     Ctl *ctl;
     u32 *buf0, *buf1;
     Edge *e0, *e1;
-    ull *delta;   // [0,V) L, [V,2V) R, [2V] ZZ; NULL = plain merge
+    ull *delta;   // [0,V) L, [V,2V) R, [2V] ZZ; NULL = plain merge.  Batched: one such vector per member
     u32 V;
     int force;
+    int batched;  // apply the ctl->nk members k_select_batch chose (bpe_train's loop); 0: the one pair (a, b)
     const unsigned char *xbase;   // sharded loop: the rank's exchange block (k_xchg.cuh); the delta vector is then
     u64 xstride;                  // the one of the current round's parity inside it, and `delta` is ignored
 };
 
-// one row (128 tokens, 4 per lane): merge starts m, kept tokens, replaced tokens written back to t[]
-template <int R>
-__device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, u32 a, u32 b, u32 z, u32 (&t)[4], u32 &mn, u32 &keep,
-                                         u32 &dirty) {
+// one row (128 tokens, 4 per lane): merge starts m, kept tokens, replaced tokens written back to t[].
+// BATCH: the nk members at mem_a instead of (a, b) -> z; member j becomes z + j.
+template <int R, bool BATCH>
+__device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, u32 a, u32 b, u32 z, u32 nk, u32 mem_a, u32 (&t)[4],
+                                         u32 &mn, u32 &keep, u32 &dirty) {
     const uint4 q = lds128o<R * 512>(la);
     const u32 nx = lds32o<R * 512 + 16>(la), pv = lds32o<R * 512 - 4>(la);
     t[0] = q.x; t[1] = q.y; t[2] = q.z; t[3] = q.w;
-    u32 m = 0;
-    m |= (((t[0] ^ a) & TOK_MASK) == 0 && t[1] == b) ? 1u : 0u;
-    m |= (((t[1] ^ a) & TOK_MASK) == 0 && t[2] == b) ? 2u : 0u;
-    m |= (((t[2] ^ a) & TOK_MASK) == 0 && t[3] == b) ? 4u : 0u;
-    m |= (((t[3] ^ a) & TOK_MASK) == 0 && nx == b) ? 8u : 0u;
-    const u32 pm = (((pv ^ a) & TOK_MASK) == 0 && t[0] == b) ? 1u : 0u;
+    u32 m = 0, pm = 0;
+#pragma unroll 1
+    for (u32 j = 0; j < (BATCH ? nk : 1u); ++j) {
+        if (BATCH) { a = lds32(mem_a + 8 * j); b = lds32(mem_a + 8 * j + 4); }
+        m |= (((t[0] ^ a) & TOK_MASK) == 0 && t[1] == b) ? 1u : 0u;
+        m |= (((t[1] ^ a) & TOK_MASK) == 0 && t[2] == b) ? 2u : 0u;
+        m |= (((t[2] ^ a) & TOK_MASK) == 0 && t[3] == b) ? 4u : 0u;
+        m |= (((t[3] ^ a) & TOK_MASK) == 0 && nx == b) ? 8u : 0u;
+        pm |= (((pv ^ a) & TOK_MASK) == 0 && t[0] == b) ? 1u : 0u;
+    }
     const u32 d = ((m << 1) | pm) & 0xfu;   // dropped: the token after a merge start
     u32 valid = 0xfu;
     if (R * 128u + 128u > count) {          // warp-uniform: the row that holds the end of the segment
@@ -108,10 +149,11 @@ __device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, u32 a, u32
     keep = ~d & valid;
     dirty |= (mn | (keep ^ valid)) ? (1u << R) : 0u;
     if (mn) {                               // few lanes: the merged token takes its place in the registers
-        if (mn & 1u) t[0] = z | (t[0] & TOK_FLAG);
-        if (mn & 2u) t[1] = z | (t[1] & TOK_FLAG);
-        if (mn & 4u) t[2] = z | (t[2] & TOK_FLAG);
-        if (mn & 8u) t[3] = z | (t[3] & TOK_FLAG);
+        auto zof = [&](u32 x) { return (BATCH ? z + batch_member(x, nk, mem_a) : z) | (x & TOK_FLAG); };
+        if (mn & 1u) t[0] = zof(t[0]);
+        if (mn & 2u) t[1] = zof(t[1]);
+        if (mn & 4u) t[2] = zof(t[2]);
+        if (mn & 8u) t[3] = zof(t[3]);
     }
 }
 
@@ -147,6 +189,7 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
     u32 *s_dkey = reinterpret_cast<u32 *>(s_bar + MS_WARPS * MS_STAGES);          // [MS_DCACHE] delta index or 0xffffffff
     u32 *s_dcnt = s_dkey + MS_DCACHE;                                             // [MS_DCACHE]
     ull *s_drops = reinterpret_cast<ull *>(s_dcnt + MS_DCACHE);
+    u32 *s_mem = reinterpret_cast<u32 *>(s_drops + 1);                            // [BATCH_MAX][2] members of a batched pass
 
     const u32 FULL = 0xffffffffu;
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -156,6 +199,8 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
     Edge *__restrict__ e_next = ctl->edge_cur ? A.e0 : A.e1;
     const u32 a = (u32)ctl->a, b = (u32)ctl->b, z = (u32)ctl->z;
     const u32 nseg = ctl->nseg;
+    const u32 nk = (!LIST && A.batched) ? ctl->nk : 1u;   // block-uniform
+    const u32 mem_a = smem_addr(s_mem);
     ull *const delta = A.xbase ? x_local_delta(A.xbase, A.xstride) : A.delta;
     const u32 *__restrict__ cand = LIST ? reinterpret_cast<const u32 *>(ctl->cand_ptr) : nullptr;
     const u32 n_cand = LIST ? ctl->n_cand : 0u;
@@ -172,6 +217,7 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
     }
     for (u32 i = tid; i < MS_DCACHE; i += MS_THREADS) { s_dkey[i] = 0xffffffffu; s_dcnt[i] = 0; }
     if (tid == 0) *s_drops = 0;
+    if (tid < nk) { s_mem[2 * tid] = tid ? (u32)ctl->bat_a[tid] : a; s_mem[2 * tid + 1] = tid ? (u32)ctl->bat_b[tid] : b; }
     __syncthreads();
 
     // ---- issue side: next non-empty segment of this warp -> bulk copy into `stage` ----
@@ -275,10 +321,17 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
         u32 t[4][4], mn[4] = {0, 0, 0, 0}, keep[4] = {0, 0, 0, 0};
         u32 dirty = 0;
         const u32 la = s_a + lane * 16;
-        mark_row<0>(la, lane, count, a, b, z, t[0], mn[0], keep[0], dirty);
-        if (count > 128u) mark_row<1>(la, lane, count, a, b, z, t[1], mn[1], keep[1], dirty);
-        if (count > 256u) mark_row<2>(la, lane, count, a, b, z, t[2], mn[2], keep[2], dirty);
-        if (count > 384u) mark_row<3>(la, lane, count, a, b, z, t[3], mn[3], keep[3], dirty);
+        if (nk == 1u) {
+            mark_row<0, false>(la, lane, count, a, b, z, 1u, mem_a, t[0], mn[0], keep[0], dirty);
+            if (count > 128u) mark_row<1, false>(la, lane, count, a, b, z, 1u, mem_a, t[1], mn[1], keep[1], dirty);
+            if (count > 256u) mark_row<2, false>(la, lane, count, a, b, z, 1u, mem_a, t[2], mn[2], keep[2], dirty);
+            if (count > 384u) mark_row<3, false>(la, lane, count, a, b, z, 1u, mem_a, t[3], mn[3], keep[3], dirty);
+        } else {
+            mark_row<0, true>(la, lane, count, a, b, z, nk, mem_a, t[0], mn[0], keep[0], dirty);
+            if (count > 128u) mark_row<1, true>(la, lane, count, a, b, z, nk, mem_a, t[1], mn[1], keep[1], dirty);
+            if (count > 256u) mark_row<2, true>(la, lane, count, a, b, z, nk, mem_a, t[2], mn[2], keep[2], dirty);
+            if (count > 384u) mark_row<3, true>(la, lane, count, a, b, z, nk, mem_a, t[3], mn[3], keep[3], dirty);
+        }
         dirty = __reduce_or_sync(FULL, dirty);   // rows in which some token is replaced or dropped
         if (!dirty) {
             // untouched segment: nothing to write, the edge record carries over
@@ -294,7 +347,9 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
             while (mall) {   // one pass per merge start of this lane
                 const int bit = __ffs(mall) - 1;
                 mall &= mall - 1;
-                delta_one(la + (bit >> 2) * 512 + (bit & 3) * 4, a, b, A.V, s_dkey, s_dcnt, delta);
+                const u32 at = la + (bit >> 2) * 512 + (bit & 3) * 4;
+                if (nk == 1u) delta_one(at, a, b, A.V, s_dkey, s_dcnt, delta);
+                else delta_batch(at, nk, mem_a, z, A.V, s_dkey, s_dcnt, delta);
             }
         }
 
@@ -363,7 +418,7 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
             ctl->n = n - dropped;
             ctl->drops = 0;
             ctl->edge_cur ^= 1u;
-            ctl->iter += 1;
+            ctl->iter += nk;
             ctl->epoch += 1;
             ctl->merge_ticket = 0; ctl->merge_exit = 0;
         }

@@ -307,12 +307,129 @@ __global__ void __launch_bounds__(256) k_argmax(Table t, Ctl *ctl, Best *partial
         ctl->best_count = r.count; ctl->best_slot = r.slot; ctl->n_tied = r.tied;
         ctl->found_pos = POS_NONE;
         ctl->tie_local = 0;
-        if (r.count == 0) ctl->done = 1;                    // max({}) -> ValueError in the reference
+        ctl->nk = 1;                                        // k_select_batch may add members
+        if (r.count == 0) ctl->done = 1;                   // max({}) -> ValueError in the reference
         else if (r.tied == 1) {
             const u64 key = t.keys[r.slot];
             record_selection(ctl, (int)(key >> 32), (int)(key & 0xffffffffu), r.count, log_pairs, log_counts);
         }
     }
+}
+
+// =============================================================================================
+// Batched merges (DESIGN.md "Batched merges").  With the pairs of the table sorted by count, p1 = the arg-max, the next
+// k merges are exactly p1 .. pk, in that order, when c1 > c2 > ... > ck > c(k+1), every pj has two different ids and
+// the 2k ids are all distinct.  A merge only lowers counts of pairs that share an id with it, and every pair it creates
+// has at most the count of such a pair, which is not a member: at most c(k+1).  So each member stays the unique maximum
+// until its turn, with the count it has now, and no tie-break is involved.  Being token-disjoint, the members never
+// overlap in the stream: one pass of k_merge_seg applies all of them.
+// k_select_batch runs after k_argmax when the arg-max is unique and a != b: the top BATCH_MAX+1 entries of the table
+// (per-thread lists, warp merge, one list per block, the last block merges the blocks' lists), then the rule above.
+// =============================================================================================
+#define TOPN (BATCH_MAX + 1)
+struct TopList { u64 c[TOPN]; u64 s[TOPN]; };   // count, slot; descending count, then ascending slot; count 0 = empty
+
+__device__ __forceinline__ bool top_before(u64 c, u64 s, u64 c2, u64 s2) { return c > c2 || (c == c2 && s < s2); }
+
+__device__ __forceinline__ void top_insert(TopList &l, u64 c, u64 s) {
+    if (!c || !top_before(c, s, l.c[TOPN - 1], l.s[TOPN - 1])) return;
+#pragma unroll
+    for (int i = TOPN - 1; i >= 0; --i) {
+        if (i > 0 && top_before(c, s, l.c[i - 1], l.s[i - 1])) { l.c[i] = l.c[i - 1]; l.s[i] = l.s[i - 1]; }
+        else { l.c[i] = c; l.s[i] = s; break; }
+    }
+}
+
+__device__ __forceinline__ void top_clear(TopList &l) {
+#pragma unroll
+    for (int i = 0; i < TOPN; ++i) { l.c[i] = 0; l.s[i] = POS_NONE; }
+}
+
+// the warp's TOPN best entries, on every lane: TOPN rounds of "best head of all lanes, its lane pops it"
+__device__ __forceinline__ TopList top_warp_merge(TopList l) {
+    TopList r;
+#pragma unroll
+    for (int k = 0; k < TOPN; ++k) {
+        u64 c = l.c[0], s = l.s[0];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const u64 c2 = __shfl_xor_sync(0xffffffffu, c, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+            if (top_before(c2, s2, c, s)) { c = c2; s = s2; }
+        }
+        r.c[k] = c; r.s[k] = s;
+        if (c && l.c[0] == c && l.s[0] == s) {   // slots are unique: exactly one lane holds the winner
+#pragma unroll
+            for (int i = 0; i + 1 < TOPN; ++i) { l.c[i] = l.c[i + 1]; l.s[i] = l.s[i + 1]; }
+            l.c[TOPN - 1] = 0; l.s[TOPN - 1] = POS_NONE;
+        }
+    }
+    return r;
+}
+
+// block-wide: every thread's list -> thread 0's list (s_l: [8] lists of shared memory)
+__device__ __forceinline__ TopList top_block_merge(TopList l, TopList *s_l) {
+    l = top_warp_merge(l);
+    if (lane_id() == 0) s_l[threadIdx.x >> 5] = l;
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+            for (int i = 0; i < TOPN; ++i) top_insert(l, s_l[w].c[i], s_l[w].s[i]);
+    return l;
+}
+
+__global__ void __launch_bounds__(256) k_select_batch(Table t, Ctl *ctl, TopList *partials, int *log_pairs, long long *log_counts) {
+    if (ctl->done || ctl->overflow || ctl->iter + 1 >= ctl->max_iter || ctl->n_tied != 1 || ctl->a == ctl->b) return;
+    const u64 cap = t.mask + 1;
+    TopList l;
+    top_clear(l);
+    const ulonglong2 *c2 = reinterpret_cast<const ulonglong2 *>(t.counts);
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < cap / 2; i += (u64)gridDim.x * blockDim.x) {
+        const ulonglong2 c = c2[i];
+        top_insert(l, c.x, 2 * i);
+        top_insert(l, c.y, 2 * i + 1);
+    }
+    __shared__ TopList s_l[8];
+    __shared__ bool last;
+    l = top_block_merge(l, s_l);
+    if (threadIdx.x == 0) {
+        partials[blockIdx.x] = l;
+        __threadfence();
+        last = (atomicAdd(&ctl->argmax_exit, 1u) == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    top_clear(l);
+    for (u32 k = threadIdx.x; k < gridDim.x * TOPN; k += blockDim.x) {
+        const TopList *p = &partials[k / TOPN];
+        top_insert(l, ld_volatile_u64(&p->c[k % TOPN]), ld_volatile_u64(&p->s[k % TOPN]));
+    }
+    __syncthreads();   // s_l is reused
+    l = top_block_merge(l, s_l);
+    if (threadIdx.x != 0) return;
+    ctl->argmax_exit = 0;
+    s_l[0] = l;   // indexed with a run-time member number below: from shared memory, so that `l` stays in registers
+    const TopList &L = s_l[0];
+    if (L.s[0] != ctl->best_slot) return;   // cannot happen: the table did not change since k_argmax
+    const u32 limit = min((u32)BATCH_MAX, ctl->max_iter - ctl->iter);
+    u32 ids[2 * BATCH_MAX];
+    ids[0] = (u32)ctl->a; ids[1] = (u32)ctl->b;
+    u32 k = 1;   // c1 > c2 holds: the arg-max is unique
+    for (; k < limit; ++k) {
+        if (!(L.c[k] > L.c[k + 1])) break;   // c(k+1) must stay below the new member's count
+        const u64 key = t.keys[L.s[k]];
+        const u32 x = (u32)(key >> 32), y = (u32)(key & 0xffffffffu);
+        bool ok = x != y;
+        for (u32 i = 0; i < 2 * k; ++i) ok = ok && ids[i] != x && ids[i] != y;
+        if (!ok) break;
+        ids[2 * k] = x; ids[2 * k + 1] = y;
+        ctl->bat_a[k] = (int)x; ctl->bat_b[k] = (int)y;
+        if (log_pairs) {
+            const u32 it = ctl->iter + k;
+            log_pairs[2 * it] = (int)x; log_pairs[2 * it + 1] = (int)y; log_counts[it] = (long long)L.c[k];
+        }
+    }
+    ctl->nk = k;
 }
 
 // =============================================================================================
@@ -441,12 +558,17 @@ __device__ __forceinline__ bool table_reserve(Ctl *ctl) {
     return false;
 }
 
+// Member j > 0 of a batched pass (use_ctl only) is a launch of its own, after member j-1's: its left and right
+// neighbours may be ids an earlier member created, whose pairs that member's launch inserts.
 __global__ void __launch_bounds__(256) k_apply_delta(Table t, Ctl *ctl, ull *__restrict__ delta, u32 V,
-                                                     int a_arg, int b_arg, int z_arg, int use_ctl, int retry) {
+                                                     int a_arg, int b_arg, int z_arg, int use_ctl, int retry, int member = 0) {
     if (use_ctl && (ctl->done || ctl->iter > ctl->max_iter)) return;
     if (use_ctl && ctl->overflow && !retry) return;   // an earlier iteration is waiting for the host
-    const u32 a = use_ctl ? (u32)ctl->a : (u32)a_arg, b = use_ctl ? (u32)ctl->b : (u32)b_arg,
-              z = use_ctl ? (u32)ctl->z : (u32)z_arg;
+    if (member > 0 && (!use_ctl || (u32)member >= ctl->nk)) return;
+    const u32 a = use_ctl ? (u32)(member ? ctl->bat_a[member] : ctl->a) : (u32)a_arg,
+              b = use_ctl ? (u32)(member ? ctl->bat_b[member] : ctl->b) : (u32)b_arg,
+              z = use_ctl ? (u32)ctl->z + (u32)member : (u32)z_arg;
+    delta += (u64)member * (2ull * V + 1);
     const u64 kab = pack_pair(a, b);
     const u32 x = blockIdx.x * blockDim.x + threadIdx.x;
     if (x < V) {
