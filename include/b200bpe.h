@@ -66,6 +66,30 @@ int bpe_load_stream(bpe_handle *h, const uint8_t *bytes, uint64_t n,
 int bpe_load_ids(bpe_handle *h, const int32_t *ids, uint64_t n,
                  const uint64_t *chunk_offsets, uint64_t n_chunks);
 
+/* Training on the distinct chunks of a text with their counts (regex.py:49-66 gives the same merges, counts and
+ * tie-breaks).  A WEIGHTED stream is a list of entries: chunk occurrences of the text, in text order, each with a weight
+ * >= 1 = the number of occurrences of the same bytes it stands for.  Every occurrence of the text must be counted by
+ * exactly one entry with the same bytes at or before it (so the first occurrence of every distinct chunk is an entry).
+ * bytes / chunk_offsets describe the entries as bpe_load_stream's arguments do; weights[n_chunks], zero is BPE_ERR_ARG.
+ * On a weighted stream bpe_train, bpe_replay, bpe_read_stream and bpe_debug_table work; bpe_get_stats, bpe_merge, the
+ * bpe_step_* / bpe_xchg_* calls, and bpe_train with BPE_OPT_RESCAN or BPE_OPT_SEG_FILTER != 0 return BPE_ERR_STATE.  Any
+ * other load makes the handle's stream unweighted again. */
+int bpe_load_chunks_weighted(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *chunk_offsets,
+                             uint64_t n_chunks, const uint64_t *weights);
+/* The same state from a text: split on the device as bpe_load_text_gpt4 does (BPE_OPT_SPLIT_PATTERN), its distinct
+ * chunks counted on the device (k_dedup.cuh).  Any length, in the splitter's pieces; HBM use grows with the distinct
+ * content of the text plus one piece, not with the text.  A chunk longer than 48 bytes, or one that finds no room in the
+ * chunk table, is an entry of weight 1 of its own.  *n_chunks = chunks of the text, *n_entries = entries (either may be
+ * NULL). */
+int bpe_load_text_gpt4_dedup(bpe_handle *h, const uint8_t *bytes, uint64_t n, uint64_t *n_chunks, uint64_t *n_entries);
+/* Counters of the last bpe_load_text_gpt4_dedup: out[0] chunks of the text, [1] entries, [2] entries from the table,
+ * [3] entries passed through (longer than 48 bytes, or no room in the table), [4] bytes of the weighted stream,
+ * [5] table slots used, [6] table slots, [7] pieces. */
+int bpe_dedup_stats(bpe_handle *h, uint64_t *out /* [8] */);
+/* The entries' weights in stream order (bpe_read_stream returns their ids).  *n = number of entries;
+ * BPE_ERR_CAPACITY if cap < *n; BPE_ERR_STATE if the stream is not weighted. */
+int bpe_read_chunk_weights(bpe_handle *h, uint64_t *out, uint64_t cap, uint64_t *n);
+
 /* Current stream length in tokens. */
 int bpe_stream_len(bpe_handle *h, uint64_t *n);
 /* Copy the current stream (ids only, chunk marks stripped) to out[0..cap).  *n = length;
@@ -270,6 +294,7 @@ int bpe_get_timing(bpe_handle *h, bpe_timing *out);
 #define BPE_OPT_SEG_FILTER 10   /* bpe_train: skip the segments a merge cannot touch (per-segment id signatures + candidate list,
                                    k_seg_filter.cuh): 0 = off (default), 1 = from the batch after merges have become sparse
                                    (fewer replacements per merge than a 32nd of the segments), 2 = always */
+#define BPE_OPT_DEDUP_LOG2 11   /* test hook: log2 of the slots of the chunk table of bpe_load_text_gpt4_dedup (0 = default 22) */
 int bpe_set_option(bpe_handle *h, int opt, int64_t value);
 
 /* Test hook: live entries (count > 0) of the incrementally maintained pair-count table, in no

@@ -24,8 +24,10 @@
 #include "k_xchg.cuh"
 #include "k_encode2.cuh"
 #include "k_special.cuh"
+#include "k_weighted.cuh"
+#include "k_dedup.cuh"
 
-#define BPE_ABI_VERSION 1
+#define BPE_ABI_VERSION 2
 
 struct EncState;
 struct SpecSet;
@@ -46,6 +48,10 @@ struct bpe_handle {
     u64 cap_tokens = 0;
     bool loaded = false;
     bool bytes_only = false;  // every id < 256 (fresh byte stream)
+    // weighted stream (bpe_load_chunks_weighted, k_weighted.cuh): one weight per entry, the entry base of every segment
+    bool weighted = false;
+    u64 *wts = nullptr; u64 wts_cap = 0, n_entries = 0;
+    u32 *wt_cnt = nullptr; u64 *wt_base = nullptr; u64 wt_seg_cap = 0;
 
     Ctl *ctl = nullptr;    // device
     Ctl *h_ctl = nullptr;  // pinned host mirror
@@ -87,6 +93,8 @@ struct bpe_handle {
     int opt_seg_filter = 0;      // BPE_OPT_SEG_FILTER: 0 = off, 1 = switch it on when merges have become sparse, 2 = always
     int opt_hist_kernel = 2;     // BPE_OPT_HIST_KERNEL: 2 = k_hist_dense (default), 1 = k_hist_dense_packed,
                                  // 0 = decide at the first large stream (cross-check + timing)
+    int opt_dedup_log2 = 0;      // BPE_OPT_DEDUP_LOG2 (test hook): log2 slots of the chunk table of bpe_load_text_gpt4_dedup, 0 = default
+    u64 dd_stats[8] = {};        // bpe_dedup_stats of the last bpe_load_text_gpt4_dedup
     int opt_split_pattern = 0;   // BPE_OPT_SPLIT_PATTERN: 0 = GPT-4 split pattern, 1 = GPT-2 (bpe_split_gpt4 / bpe_load_text_gpt4 / bpe_encode_text_gpt4*)
 
     bpe_timing tm = {};
@@ -226,6 +234,9 @@ extern "C" int bpe_destroy(bpe_handle *h) {
     if (h->d_cls) cudaFree(h->d_cls);
     if (h->d_contr) cudaFree(h->d_contr);
     if (h->d_present) cudaFree(h->d_present);
+    if (h->wts) cudaFree(h->wts);
+    if (h->wt_cnt) cudaFree(h->wt_cnt);
+    if (h->wt_base) cudaFree(h->wt_base);
     xchg_release(h);
     enc2_free(h);
     spec_free(h);
@@ -269,6 +280,9 @@ extern "C" int bpe_set_option(bpe_handle *h, int opt, int64_t value) {
         case BPE_OPT_SPLIT_PATTERN:
             if (value != 0 && value != 1) return fail(h, BPE_ERR_ARG, "split pattern must be 0 (GPT-4) or 1 (GPT-2)");
             h->opt_split_pattern = (int)value; break;
+        case BPE_OPT_DEDUP_LOG2:
+            if (value != 0 && (value < 4 || value > 30)) return fail(h, BPE_ERR_ARG, "dedup log2 must be 0 or in [4,30]");
+            h->opt_dedup_log2 = (int)value; break;
         case BPE_OPT_SPLIT_PIECE:
             if (value != 0 && value < 4096) return fail(h, BPE_ERR_ARG, "split piece must be 0 (default) or >= 4096 bytes");
             g_split_piece_override = (u64)value; break;
@@ -332,6 +346,13 @@ static void enqueue_pack(bpe_handle *h, int force) {
 static void enqueue_edges_after_contig(bpe_handle *h) {
     k_build_edges<<<h->sms * 4, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], 1);
     h->tm.kernel_launches += 1;
+}
+
+// entry base of every segment of a weighted stream (k_weighted.cuh); force = 0: only if the stream was just packed
+static void enqueue_wt_bases(bpe_handle *h, int force) {
+    k_wt_marks<<<h->sms * 8, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], h->wt_cnt, force);
+    k_wt_scan<<<1, 1024, 0, h->stream>>>(h->ctl, h->wt_cnt, h->wt_base, force);
+    h->tm.kernel_launches += 2;
 }
 
 static int push_ctl(bpe_handle *h) {
@@ -414,7 +435,7 @@ extern "C" int bpe_load_stream(bpe_handle *h, const uint8_t *bytes, uint64_t n, 
     int rc = check_offsets(h, chunk_offsets, n_chunks, n);
     if (rc) return rc;
     h->tm.h2d_bytes = 0;
-    h->loaded = false; h->table_valid = false;
+    h->loaded = false; h->table_valid = false; h->weighted = false;
     if ((rc = ensure_stream_capacity(h, n))) return rc;
     if ((rc = load_bytes_into(h, h->buf[0], bytes, n, nullptr))) return rc;
     if ((rc = mark_chunks(h, h->buf[0], chunk_offsets, n_chunks, n))) return rc;
@@ -433,7 +454,7 @@ extern "C" int bpe_load_ids(bpe_handle *h, const int32_t *ids, uint64_t n, const
     int rc = check_offsets(h, chunk_offsets, n_chunks, n);
     if (rc) return rc;
     h->tm.h2d_bytes = 0;
-    h->loaded = false; h->table_valid = false;
+    h->loaded = false; h->table_valid = false; h->weighted = false;
     if ((rc = ensure_stream_capacity(h, n))) return rc;
     h->max_id = 0;
     if (n) {
@@ -490,10 +511,79 @@ extern "C" int bpe_read_stream(bpe_handle *h, int32_t *out, uint64_t cap, uint64
 }
 
 // ------------------------------------------------------------------------------------------------
+// weighted stream (k_weighted.cuh): entries = chunk occurrences in text order, each standing for `weight` occurrences
+// storage of a weighted stream of n_entries entries over the stream just loaded (its segments: h->seg_cap)
+static int wt_alloc(bpe_handle *h, u64 n_entries) {
+    if (n_entries > h->wts_cap) {
+        if (h->wts) cudaFree(h->wts);
+        h->wts = nullptr; h->wts_cap = 0;
+        CU(cudaMalloc(&h->wts, n_entries * 8));
+        h->wts_cap = n_entries;
+    }
+    if (h->seg_cap > h->wt_seg_cap) {
+        if (h->wt_cnt) cudaFree(h->wt_cnt);
+        if (h->wt_base) cudaFree(h->wt_base);
+        h->wt_cnt = nullptr; h->wt_base = nullptr; h->wt_seg_cap = 0;
+        CU(cudaMalloc(&h->wt_cnt, h->seg_cap * 4));
+        CU(cudaMalloc(&h->wt_base, h->seg_cap * 8));
+        h->wt_seg_cap = h->seg_cap;
+    }
+    return BPE_OK;
+}
+// the weights are in h->wts: entry bases, and the handle holds a weighted stream
+static int wt_finish(bpe_handle *h, u64 n_entries) {
+    enqueue_wt_bases(h, 1);
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(h->stream));
+    h->n_entries = n_entries;
+    h->weighted = true; h->loaded = true;
+    return BPE_OK;
+}
+
+extern "C" int bpe_load_chunks_weighted(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *chunk_offsets,
+                                        uint64_t n_chunks, const uint64_t *weights) {
+    if (!h) return BPE_ERR_ARG;
+    if (n && (!chunk_offsets || !n_chunks)) return fail(h, BPE_ERR_ARG, "bpe_load_chunks_weighted: a non-empty text needs chunk offsets");
+    if (!n && n_chunks) return fail(h, BPE_ERR_ARG, "bpe_load_chunks_weighted: chunks of an empty text");
+    if (n_chunks && !weights) return fail(h, BPE_ERR_ARG, "weights is NULL");
+    for (u64 i = 0; i < n_chunks; ++i)
+        if (weights[i] == 0) return fail(h, BPE_ERR_ARG, "weights must be >= 1");
+    int rc = bpe_load_stream(h, bytes, n, chunk_offsets, n_chunks);   // validates the rest; leaves an unweighted stream
+    if (rc) return rc;
+    h->loaded = false;
+    if ((rc = wt_alloc(h, n_chunks))) return rc;
+    if (n_chunks) CU(cudaMemcpyAsync(h->wts, weights, n_chunks * 8, cudaMemcpyHostToDevice, h->stream));
+    h->tm.h2d_bytes += n_chunks * 8;
+    return wt_finish(h, n_chunks);   // synchronises: `weights` is the caller's buffer
+}
+
+extern "C" int bpe_read_chunk_weights(bpe_handle *h, uint64_t *out, uint64_t cap, uint64_t *n) {
+    if (!h || !n) return BPE_ERR_ARG;
+    if (!h->loaded) return fail(h, BPE_ERR_STATE, "no stream loaded");
+    if (!h->weighted) return fail(h, BPE_ERR_STATE, "bpe_read_chunk_weights: the loaded stream is not weighted");
+    *n = h->n_entries;
+    if (cap < h->n_entries) return fail(h, BPE_ERR_CAPACITY, "output buffer too small");
+    if (!h->n_entries) return BPE_OK;
+    if (!out) return fail(h, BPE_ERR_ARG, "out is NULL");
+    CU(cudaSetDevice(h->device));
+    CU(cudaMemcpyAsync(out, h->wts, h->n_entries * 8, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->tm.d2h_bytes = h->n_entries * 8;
+    return BPE_OK;
+}
+
+// the sharded loop (step_host.inl) has no weighted form
+static int refuse_weighted(bpe_handle *h, const char *what) {
+    return h->weighted ? fail(h, BPE_ERR_STATE, std::string(what) + ": not available on a weighted stream (bpe_load_chunks_weighted)")
+                       : BPE_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // get_stats (base.py:13-22)
 extern "C" int bpe_get_stats(bpe_handle *h, int32_t *pairs, int64_t *counts, uint64_t cap, uint64_t *n_pairs) {
     if (!h || !n_pairs) return BPE_ERR_ARG;
     if (!h->loaded) return fail(h, BPE_ERR_STATE, "no stream loaded");
+    if (h->weighted) return fail(h, BPE_ERR_STATE, "bpe_get_stats: not available on a weighted stream (bpe_load_chunks_weighted)");
     CU(cudaSetDevice(h->device));
     int rc = pull_ctl(h);
     if (rc) return rc;
@@ -540,9 +630,18 @@ extern "C" int bpe_get_stats(bpe_handle *h, int32_t *pairs, int64_t *counts, uin
 // the whole sequence is enqueued unconditionally; `same` >= 0 lets the host skip the no-ops when
 // it knows the pair (single-step API).
 // `batched`: the pass applies the members k_select_batch chose (bpe_train's loop only; a pair (a,a) is never batched).
+// Weighted stream (k_weighted.cuh): the weighted delta is computed by a pass of its own in front of the merge, which then
+// runs without a delta vector.
 static void launch_merge(bpe_handle *h, ull *delta, int force, int same = -1, bool use_xchg = false, bool batched = false) {
     const unsigned char *xbase = use_xchg ? h->xchg : nullptr;
+    ull *const wdelta = h->weighted ? delta : nullptr;   // weighted: the delta passes add into it ...
+    if (wdelta) delta = nullptr;                          // ... and the merge kernels below are plain merges
     if (same != 1) {
+        if (wdelta) {
+            k_wt_delta_seg<<<h->sms * 8, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], h->wt_base,
+                                                              h->wts, wdelta, h->V, batched, force);
+            h->tm.kernel_launches += 1;
+        }
         SegArgs S;
         S.ctl = h->ctl; S.buf0 = h->buf[0]; S.buf1 = h->buf[1]; S.e0 = h->edge[0]; S.e1 = h->edge[1];
         S.delta = delta; S.V = h->V; S.force = force; S.batched = batched; S.xbase = xbase; S.xstride = h->xchg_stride;
@@ -555,8 +654,18 @@ static void launch_merge(bpe_handle *h, ull *delta, int force, int same = -1, bo
         A.ctl = h->ctl; A.buf0 = h->buf[0]; A.buf1 = h->buf[1]; A.desc = h->desc; A.delta = delta; A.V = h->V; A.force = force;
         A.xbase = xbase; A.xstride = h->xchg_stride;
         enqueue_pack(h, force);
+        if (h->weighted) {            // gated on the pack having run (ctl->contig), like the edges below
+            enqueue_wt_bases(h, 0);
+            if (wdelta) {
+                const u64 nblk = (h->h_ctl->n + SEG_TOKENS - 1) / SEG_TOKENS;   // host copy: an upper bound of the device's
+                k_wt_delta_same<<<grid_for(nblk, 256, h->sms * 8), 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->wt_base,
+                                                                                       h->wts, wdelta, h->V, force);
+                h->tm.kernel_launches += 1;
+            }
+        }
         k_merge<true><<<h->merge_grid_same, MG_THREADS, 0, h->stream>>>(A);
         h->tm.kernel_launches += 1;
+        if (h->weighted) enqueue_wt_bases(h, 0);
         enqueue_edges_after_contig(h);
         if (h->filt_active) {      // the pack moved tokens between segments: signatures from the tokens again (gated on a == b)
             k_sig_build<<<h->sms * 8, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], h->sig, 1);
@@ -568,6 +677,7 @@ static void launch_merge(bpe_handle *h, ull *delta, int force, int same = -1, bo
 extern "C" int bpe_merge(bpe_handle *h, int32_t a, int32_t b, int32_t idx, uint64_t *new_len) {
     if (!h) return BPE_ERR_ARG;
     if (!h->loaded) return fail(h, BPE_ERR_STATE, "no stream loaded");
+    if (h->weighted) return fail(h, BPE_ERR_STATE, "bpe_merge: not available on a weighted stream (bpe_load_chunks_weighted)");
     if (a < 0 || b < 0 || idx < 0 || a == 0x7fffffff || b == 0x7fffffff || idx == 0x7fffffff)
         return fail(h, BPE_ERR_ARG, "ids must be in [0, 2^31-1)");
     CU(cudaSetDevice(h->device));
@@ -692,7 +802,11 @@ static int build_table(bpe_handle *h, u64 cap) {
     }
     const ull zero = 0;
     CU(cudaMemcpyAsync(&h->ctl->table_used, &zero, 8, cudaMemcpyHostToDevice, h->stream));
-    if (h->bytes_only) {
+    if (h->weighted) {      // weighted sums straight into the table; takes no part in the choice of hist_dense
+        CU(cudaMemsetAsync(h->d_err, 0, 4, h->stream));
+        k_wt_hist<<<h->sms * 8, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], h->wt_base, h->wts, h->table);
+        h->tm.kernel_launches += 1;
+    } else if (h->bytes_only) {
         CU(cudaMemsetAsync(h->dense, 0, 65536 * 8, h->stream));
         CU(cudaMemsetAsync(h->d_err, 0, 4, h->stream));
         if ((rc = hist_dense(h, h->dense))) return rc;
@@ -771,6 +885,7 @@ static void maybe_repack(bpe_handle *h) {
     if (nseg < 64 || h->h_ctl->contig) return;
     if (2 * h->h_ctl->n >= nseg * (u64)SEG_TOKENS) return;
     enqueue_pack(h, 1);
+    if (h->weighted) enqueue_wt_bases(h, 0);
     enqueue_edges_after_contig(h);
     if (h->filt_active) {
         k_sig_build<<<h->sms * 8, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], h->sig, 0);
@@ -851,6 +966,8 @@ extern "C" int bpe_train(bpe_handle *h, int32_t num_merges, int32_t first_idx, i
     if (num_merges < 0 || first_idx < 0) return fail(h, BPE_ERR_ARG, "num_merges and first_idx must be >= 0");
     if ((u64)first_idx + (u64)num_merges >= 0x7fffffffull) return fail(h, BPE_ERR_ARG, "vocabulary would exceed 2^31-1");
     if (num_merges && (!out_pairs || !out_counts)) return fail(h, BPE_ERR_ARG, "output buffers are NULL");
+    if (h->weighted && (h->opt_rescan || h->opt_seg_filter))
+        return fail(h, BPE_ERR_STATE, "bpe_train: BPE_OPT_RESCAN and BPE_OPT_SEG_FILTER are not available on a weighted stream");
     CU(cudaSetDevice(h->device));
     *n_done = 0;
     h->tm.kernel_launches = 0; h->tm.d2h_bytes = 0; h->tm.merge_kernel_ms = 0;
@@ -975,3 +1092,4 @@ extern "C" int bpe_debug_table(bpe_handle *h, int32_t *pairs, int64_t *counts, u
 #include "split_host.inl"
 #include "encode2_host.inl"
 #include "decode_host.inl"
+#include "dedup_host.inl"

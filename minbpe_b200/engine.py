@@ -10,9 +10,10 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
+OPT_DEDUP_LOG2 = 11
 ERR_CAPACITY = -4
 
 _lib = None
@@ -51,6 +52,10 @@ def load_library():
         "bpe_last_error": ([vp], ctypes.c_char_p),
         "bpe_load_stream": ([vp, vp, u64, vp, u64], ci),
         "bpe_load_ids": ([vp, vp, u64, vp, u64], ci),
+        "bpe_load_chunks_weighted": ([vp, vp, u64, vp, u64, vp], ci),
+        "bpe_read_chunk_weights": ([vp, vp, u64, P(u64)], ci),
+        "bpe_load_text_gpt4_dedup": ([vp, vp, u64, P(u64), P(u64)], ci),
+        "bpe_dedup_stats": ([vp, vp], ci),
         "bpe_stream_len": ([vp, P(u64)], ci),
         "bpe_read_stream": ([vp, vp, u64, P(u64)], ci),
         "bpe_get_stats": ([vp, vp, vp, u64, P(u64)], ci),
@@ -147,6 +152,29 @@ class Engine:
         a = np.ascontiguousarray(ids, dtype=np.int32)
         o, k = _as_offsets(offsets)
         self._check(self._lib.bpe_load_ids(self._h, _ptr(a) if a.size else None, a.size, _ptr(o), k), "bpe_load_ids")
+
+    def load_chunks_weighted(self, data, offsets, weights):
+        """A weighted stream (bpe_load_chunks_weighted): entries = chunk occurrences in text order (bytes back to back,
+        start offsets), weights[k] >= 1 = how many occurrences of the same bytes entry k stands for.  train() on it gives
+        the merges and counts of training on the whole text."""
+        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        o, k = _as_offsets(offsets)
+        w = np.ascontiguousarray(weights, dtype=np.uint64)
+        if w.size != k:
+            raise EngineError(f"load_chunks_weighted: {w.size} weights for {k} chunks")
+        self._keep = (b, o, w)
+        self._check(self._lib.bpe_load_chunks_weighted(self._h, _ptr(b) if b.size else None, b.size, _ptr(o), k,
+                                                       _ptr(w) if w.size else None), "bpe_load_chunks_weighted")
+
+    def chunk_weights(self):
+        """Weights of the entries of the loaded weighted stream, in stream order (uint64)."""
+        n = ctypes.c_uint64()
+        rc = self._lib.bpe_read_chunk_weights(self._h, None, 0, ctypes.byref(n))
+        if rc != ERR_CAPACITY:
+            self._check(rc, "bpe_read_chunk_weights")
+        out = np.empty(max(n.value, 1), dtype=np.uint64)
+        self._check(self._lib.bpe_read_chunk_weights(self._h, _ptr(out), out.size, ctypes.byref(n)), "bpe_read_chunk_weights")
+        return out[: n.value]
 
     def stream_len(self):
         n = ctypes.c_uint64()
@@ -307,6 +335,22 @@ class Engine:
         self._check(self._lib.bpe_load_text_gpt4(self._h, _ptr(b) if b.size else None, b.size,
                                                  ctypes.byref(n) if count_chunks else None), "bpe_load_text_gpt4")
         return n.value if count_chunks else None
+
+    def load_text_gpt4_dedup(self, data):
+        """Upload utf-8 `data`, split it on the GPU (BPE_OPT_SPLIT_PATTERN), count its distinct chunks there and make the
+        weighted stream of the distinct chunks with their counts the current stream.  -> (chunks of the text, entries)."""
+        self._ensure_gpt4_tables()
+        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        nc, ne = ctypes.c_uint64(), ctypes.c_uint64()
+        self._check(self._lib.bpe_load_text_gpt4_dedup(self._h, _ptr(b) if b.size else None, b.size, ctypes.byref(nc),
+                                                       ctypes.byref(ne)), "bpe_load_text_gpt4_dedup")
+        return nc.value, ne.value
+
+    def dedup_stats(self):
+        a = np.zeros(8, dtype=np.uint64)
+        self._check(self._lib.bpe_dedup_stats(self._h, _ptr(a)), "bpe_dedup_stats")
+        names = ("text_chunks", "entries", "table_entries", "passthrough_entries", "stream_bytes", "slots_used", "slots", "pieces")
+        return {k: int(v) for k, v in zip(names, a)}
 
     # ---- step-wise training (sharded loop; device pointers, e.g. torch tensors' data_ptr()) ----
     def set_stream(self, cuda_stream_ptr):

@@ -9,6 +9,9 @@ so callers and the reference's own tests work unchanged; the loops underneath ar
     get_stats / merge  -> Engine.get_stats / Engine.merge      (bpe_get_stats, bpe_merge)
     GPT-4 pre-split    -> Engine.load_text_gpt4 / split_gpt4   (bpe_load_text_gpt4, bpe_split_gpt4) for texts
                           of at least 64 KiB; same chunks as regex.findall (tests/test_gpu_split.py)
+    train(dedup=True)  -> Engine.load_text_gpt4_dedup (device split + device chunk counting) for the texts the device
+                          splits, else count_chunks + Engine.load_chunks_weighted; then Engine.train: the distinct
+                          chunks with their counts, same merges as the whole text
 
 What stays on the host, as in the reference: the regex pre-split for any other pattern and for
 short texts (third-party ``regex`` module, regex.py:41,114), special-token splitting
@@ -17,7 +20,9 @@ short texts (third-party ``regex`` module, regex.py:41,114), special-token split
 
 There is no CPU fallback: without libb200bpe.so and an H100 the device-backed calls raise.
 """
+import os
 import unicodedata
+from collections import Counter
 
 import numpy as np
 import regex as re
@@ -130,14 +135,20 @@ class Tokenizer:
             m[r, 0], m[r, 1] = pair
         return m
 
-    def _run_training(self, data, offsets, vocab_size, verbose, device_split=False, resume=False):
+    def _run_training(self, data, offsets, vocab_size, verbose, device_split=False, resume=False, weights=None, dedup=False):
         """Shared by Basic/Regex: basic.py:21-49 / regex.py:37-70 minus the Python loops.  resume=True (not in the
         reference): keep the merges this tokenizer already has (e.g. from load()), replay them on the text and
-        continue the same training run up to vocab_size — train(N) == train(k); save; load; train(N, resume=True)."""
+        continue the same training run up to vocab_size — train(N) == train(k); save; load; train(N, resume=True).
+        weights: the chunks are distinct chunks with these counts (count_chunks) and train as the whole text would;
+        device_split and dedup: the chunks are split and counted on the device."""
         assert vocab_size >= 256
         num_merges = vocab_size - 256
         eng = self.engine
-        if device_split:
+        if weights is not None:
+            eng.load_chunks_weighted(data, offsets, weights)
+        elif device_split and dedup:
+            eng.load_text_gpt4_dedup(data)     # split + distinct chunks counted on the GPU (k_dedup.cuh)
+        elif device_split:
             eng.load_text_gpt4(data)      # regex.py:41-44 on the GPU (k_split.cuh)
         else:
             eng.load_stream(data, offsets)
@@ -299,6 +310,23 @@ def split_text(compiled_pattern, text):
     return b"".join(enc), offs.astype(np.uint64)
 
 
+def count_chunks(data, offsets):
+    """The distinct chunks of (bytes, chunk start offsets) in first-occurrence order, with how often each occurs:
+    -> (their bytes back to back, their start offsets uint64, their counts uint64).  Pairs never cross a chunk and equal
+    chunks go through the same merges, so training on these with the counts as weights gives the merges, counts and
+    tie-breaks of training on the whole text."""
+    offs = np.asarray(offsets, dtype=np.int64)
+    if offs.size == 0:
+        return b"", np.zeros(0, dtype=np.uint64), np.zeros(0, dtype=np.uint64)
+    raw = bytes(data)
+    ends = np.append(offs[1:], len(raw))
+    counts = Counter(map(raw.__getitem__, map(slice, offs.tolist(), ends.tolist())))   # dict order = first occurrence
+    lens = np.fromiter(map(len, counts), dtype=np.int64, count=len(counts))
+    starts = np.zeros(len(counts), dtype=np.int64)
+    np.cumsum(lens[:-1], out=starts[1:])
+    return b"".join(counts), starts.astype(np.uint64), np.fromiter(counts.values(), dtype=np.uint64, count=len(counts))
+
+
 class RegexTokenizer(Tokenizer):
     """regex.py:22-164: regex pre-split into chunks; pairs and merges never cross a chunk."""
 
@@ -334,27 +362,56 @@ class RegexTokenizer(Tokenizer):
         return (0 < len(special) <= E.SPECIAL_MAX and
                 all(isinstance(k, str) and 0 < len(k.encode("utf-8")) <= E.SPECIAL_MAX_BYTES and 0 <= int(v) < 2 ** 31 for k, v in special.items()))
 
-    def train(self, text, vocab_size, verbose=False, *, resume=False):
+    def train(self, text, vocab_size, verbose=False, *, resume=False, dedup=False):
+        """regex.py:35-70.  dedup=True (not in the reference): train on the distinct chunks of the text with their counts,
+        which gives the same merges, vocab and verbose lines as dedup=False with less work per merge when chunks
+        repeat, as they do in natural text.  Texts the device splits (GPT-2 / GPT-4 patterns, at least 64 KiB) are
+        split and counted on the device (bpe_load_text_gpt4_dedup); other patterns and short texts are split with
+        `regex` and counted on the host (count_chunks)."""
         assert vocab_size >= 256
         data = text.encode("utf-8")
+        if dedup:
+            if self._device_split(len(data)):
+                self._run_training(data, None, vocab_size, verbose, device_split=True, resume=resume, dedup=True)
+                return
+            data, offsets = split_text(self.compiled_pattern, text)
+            data, offsets, weights = count_chunks(data, offsets)
+            self._run_training(data, offsets, vocab_size, verbose, resume=resume, weights=weights)
+            return
         if self._device_split(len(data)):
             self._run_training(data, None, vocab_size, verbose, device_split=True, resume=resume)
             return
         data, offsets = split_text(self.compiled_pattern, text)
         self._run_training(data, offsets, vocab_size, verbose, resume=resume)
 
-    def train_from_file(self, path, vocab_size, verbose=False, *, group=None):
+    def train_from_file(self, path, vocab_size, verbose=False, *, group=None, dedup=False):
         """train() for a UTF-8 text file of any size (not in the reference, which takes a str: regex.py:36).  The file
         is memory-mapped and split on the device in pieces; when torch.distributed is initialised (one process per
         GPU) every rank trains on its own byte range — cut where a letter is followed by a space, a provable chunk
-        boundary of both patterns — and all ranks end with identical merges / vocab.  GPT-2 / GPT-4 split patterns only."""
+        boundary of both patterns — and all ranks end with identical merges / vocab.  GPT-2 / GPT-4 split patterns only.
+        dedup=True: one GPU counts the file's distinct chunks (bpe_load_text_gpt4_dedup) and trains on them, so HBM holds
+        the distinct content rather than the file; not with a process group of more than one rank (ValueError)."""
         assert vocab_size >= 256
         which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
         if which is None:
             raise ValueError("train_from_file splits on the device and supports the GPT-2 / GPT-4 split patterns only; "
                              "use train(open(path).read(), ...) for other patterns")
-        from .dist import train_file
         from .engine import OPT_SPLIT_PATTERN
+        if dedup:
+            import torch.distributed as dist
+            if (group is not None and dist.get_world_size(group) > 1) or (dist.is_available() and dist.is_initialized()
+                                                                          and dist.get_world_size() > 1):
+                raise ValueError("train_from_file(dedup=True) runs on one GPU; sharded training does not count distinct chunks")
+            eng = self.engine
+            eng.set_option(OPT_SPLIT_PATTERN, which)
+            data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) else np.zeros(0, dtype=np.uint8)
+            eng.load_text_gpt4_dedup(data)
+            del data
+            pairs, counts, done = eng.train(vocab_size - 256)
+            self.last_timing = eng.timing()
+            self._adopt(pairs, counts, done, vocab_size - 256, verbose)
+            return
+        from .dist import train_file
         eng = self.engine
         eng.set_option(OPT_SPLIT_PATTERN, which)
         pairs, counts, done = train_file(eng, eng.device, path, vocab_size - 256, group=group)
