@@ -9,49 +9,11 @@ import pytest
 import regex
 
 import oracle
+from batch_model import merge, predict
 
 GPT4 = regex.compile(
     r"""'(?i:[sdmt]|ll|ve|re)|[^\r\n\p{L}\p{N}]?+\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]++[\r\n]*|\s*[\r\n]|\s+(?!\S)|\s+""")
 CAP = 8   # the device carries at most BATCH_MAX (4) merges per pass; a correct batch of 8 has correct prefixes
-
-
-def predict(pairs, counts, cap):
-    """The batch the rule allows at this step: [(pair, count)], empty when the arg-max is tied."""
-    if len(counts) == 0:
-        return []
-    order = np.argsort(-counts, kind="stable")
-    c = counts[order].tolist() + [0] * (cap + 1)
-    p = [tuple(x) for x in pairs[order].tolist()]
-    if c[0] == c[1] or p[0][0] == p[0][1]:
-        return []
-    ids = {p[0][0], p[0][1]}
-    k = 1
-    while k < cap and c[k] > c[k + 1]:
-        x, y = p[k]
-        if x == y or x in ids or y in ids:
-            break
-        ids |= {x, y}
-        k += 1
-    return [(p[j], c[j]) for j in range(k)]
-
-
-def merge(ids, start, pair, z):
-    """base.py:25-41 over a stream whose chunk starts are marked in `start` (no pair spans two chunks)."""
-    a, b = pair
-    hit = (ids[:-1] == a) & (ids[1:] == b) & ~start[1:]
-    pos = np.flatnonzero(hit)
-    if a == b:   # runs: greedy from the left
-        keep, last = [], -2
-        for q in pos.tolist():
-            if q != last + 1:
-                keep.append(q)
-                last = q
-        pos = np.asarray(keep, dtype=np.int64)
-    ids = ids.copy()
-    ids[pos] = z
-    drop = np.ones(len(ids), dtype=bool)
-    drop[pos + 1] = False
-    return ids[drop], start[drop]
 
 
 def check(data, offs, merges):
@@ -68,7 +30,7 @@ def check(data, offs, merges):
         for j, (pair, count) in enumerate(batch):
             assert pair == tuple(want_pairs[i + j]) and count == want_counts[i + j], (i, j, batch)
         batched += len(batch) > 1
-        ids, start = merge(ids, start, want_pairs[i], 256 + i)
+        ids, start, _ = merge(ids, start, want_pairs[i], 256 + i)
     assert np.array_equal(ids, final)   # the stepping above is the oracle's loop
     return batched
 
