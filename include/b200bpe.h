@@ -82,13 +82,30 @@ int bpe_load_chunks_weighted(bpe_handle *h, const uint8_t *bytes, uint64_t n, co
  * chunk table, is an entry of weight 1 of its own.  *n_chunks = chunks of the text, *n_entries = entries (either may be
  * NULL). */
 int bpe_load_text_gpt4_dedup(bpe_handle *h, const uint8_t *bytes, uint64_t n, uint64_t *n_chunks, uint64_t *n_entries);
-/* Counters of the last bpe_load_text_gpt4_dedup: out[0] chunks of the text, [1] entries, [2] entries from the table,
- * [3] entries passed through (longer than 48 bytes, or no room in the table), [4] bytes of the weighted stream,
- * [5] table slots used, [6] table slots, [7] pieces. */
+/* Entries built elsewhere, merged into one weighted stream on the device: the weighted streams of a text's consecutive
+ * parts (e.g. each rank's bpe_load_text_gpt4_dedup of its byte range, read back with bpe_read_chunk_entries), concatenated
+ * in text order.  Arguments and validation (and error codes) as bpe_load_chunks_weighted.  Every entry of <= 48 bytes finds
+ * or claims a slot of the chunk table (BPE_OPT_DEDUP_LOG2) by its bytes; the slot's weight is the sum of its entries'
+ * weights and its entry of smallest index is kept.  An entry without a slot (longer than 48 bytes, or no room in the table)
+ * is kept with its own weight.  When every part obeys the rule above for its own text, the result obeys it for the whole
+ * text; with no table overflow it equals bpe_load_text_gpt4_dedup of the whole text.  One pass over the whole input; HBM =
+ * the input's bytes, offsets and weights, plus the table.  *n_entries = entries kept (may be NULL). */
+int bpe_load_chunks_weighted_dedup(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *chunk_offsets,
+                                   uint64_t n_chunks, const uint64_t *weights, uint64_t *n_entries);
+/* Counters of the last bpe_load_text_gpt4_dedup or bpe_load_chunks_weighted_dedup: out[0] chunks of the text (the merge:
+ * the sum of the input weights), [1] entries, [2] entries from the table, [3] entries passed through (longer than 48 bytes,
+ * or no room in the table), [4] bytes of the weighted stream, [5] table slots used, [6] table slots, [7] pieces (the
+ * merge: 0). */
 int bpe_dedup_stats(bpe_handle *h, uint64_t *out /* [8] */);
 /* The entries' weights in stream order (bpe_read_stream returns their ids).  *n = number of entries;
  * BPE_ERR_CAPACITY if cap < *n; BPE_ERR_STATE if the stream is not weighted. */
 int bpe_read_chunk_weights(bpe_handle *h, uint64_t *out, uint64_t cap, uint64_t *n);
+/* The entries of the loaded weighted stream: their bytes back to back in bytes[0..*n_bytes) and their start offsets in
+ * offsets[0..*n_entries) (bpe_read_stream strips the chunk marks).  Sizes are always reported; BPE_ERR_CAPACITY if
+ * cap_bytes < *n_bytes or cap_entries < *n_entries (so cap = 0 asks for them).  BPE_ERR_STATE if the stream is not
+ * weighted, or once bpe_train / bpe_replay has run on it. */
+int bpe_read_chunk_entries(bpe_handle *h, uint8_t *bytes, uint64_t cap_bytes, uint64_t *offsets, uint64_t cap_entries,
+                           uint64_t *n_bytes, uint64_t *n_entries);
 
 /* Current stream length in tokens. */
 int bpe_stream_len(bpe_handle *h, uint64_t *n);
@@ -294,7 +311,8 @@ int bpe_get_timing(bpe_handle *h, bpe_timing *out);
 #define BPE_OPT_SEG_FILTER 10   /* bpe_train: skip the segments a merge cannot touch (per-segment id signatures + candidate list,
                                    k_seg_filter.cuh): 0 = off (default), 1 = from the batch after merges have become sparse
                                    (fewer replacements per merge than a 32nd of the segments), 2 = always */
-#define BPE_OPT_DEDUP_LOG2 11   /* test hook: log2 of the slots of the chunk table of bpe_load_text_gpt4_dedup (0 = default 22) */
+#define BPE_OPT_DEDUP_LOG2 11   /* test hook: log2 of the slots of the chunk table of bpe_load_text_gpt4_dedup and
+                                   bpe_load_chunks_weighted_dedup (0 = default 22) */
 int bpe_set_option(bpe_handle *h, int opt, int64_t value);
 
 /* Test hook: live entries (count > 0) of the incrementally maintained pair-count table, in no

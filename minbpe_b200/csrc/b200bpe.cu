@@ -27,7 +27,7 @@
 #include "k_weighted.cuh"
 #include "k_dedup.cuh"
 
-#define BPE_ABI_VERSION 2
+#define BPE_ABI_VERSION 3
 
 struct EncState;
 struct SpecSet;
@@ -52,6 +52,7 @@ struct bpe_handle {
     bool weighted = false;
     u64 *wts = nullptr; u64 wts_cap = 0, n_entries = 0;
     u32 *wt_cnt = nullptr; u64 *wt_base = nullptr; u64 wt_seg_cap = 0;
+    bool wt_fresh = false;    // the weighted stream is as loaded: no bpe_train / bpe_replay since (bpe_read_chunk_entries)
 
     Ctl *ctl = nullptr;    // device
     Ctl *h_ctl = nullptr;  // pinned host mirror
@@ -536,7 +537,7 @@ static int wt_finish(bpe_handle *h, u64 n_entries) {
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(h->stream));
     h->n_entries = n_entries;
-    h->weighted = true; h->loaded = true;
+    h->weighted = true; h->loaded = true; h->wt_fresh = true;
     return BPE_OK;
 }
 
@@ -968,6 +969,7 @@ extern "C" int bpe_train(bpe_handle *h, int32_t num_merges, int32_t first_idx, i
     if (num_merges && (!out_pairs || !out_counts)) return fail(h, BPE_ERR_ARG, "output buffers are NULL");
     if (h->weighted && (h->opt_rescan || h->opt_seg_filter))
         return fail(h, BPE_ERR_STATE, "bpe_train: BPE_OPT_RESCAN and BPE_OPT_SEG_FILTER are not available on a weighted stream");
+    h->wt_fresh = false;
     CU(cudaSetDevice(h->device));
     *n_done = 0;
     h->tm.kernel_launches = 0; h->tm.d2h_bytes = 0; h->tm.merge_kernel_ms = 0;

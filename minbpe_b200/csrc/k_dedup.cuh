@@ -1,15 +1,19 @@
 // k_dedup.cuh — counting the distinct chunks of a text on the device (bpe_load_text_gpt4_dedup, dedup_host.inl).
 //
 // Per piece of the text (the splitter's pieces), with the chunk starts of the piece compacted to offsets:
-//   k_dd_count  every chunk of <= DD_KEY_MAX bytes claims or finds a slot of the chunk table (exact byte compare; a
-//               slot's key is published before its tag, so nobody compares against a half-written key), adds 1 to the
+//   k_dd_count<false>  every chunk of <= DD_KEY_MAX bytes claims or finds a slot of the chunk table (exact byte compare;
+//               a slot's key is published before its tag, so nobody compares against a half-written key), adds 1 to the
 //               slot's count and atomicMin's its text position into the slot's first position
 //   k_dd_keep   an occurrence is kept as an entry when it is its slot's first occurrence, or when it has no slot
 //               (longer than the key, or no free slot within DD_PROBES probes): the rule of DESIGN.md §14
 //   k_dd_lens / k_dd_scan_u64 / k_dd_emit   the kept chunks' bytes, offsets and slots appended to the output, in text order
 // A slot's first position is final once its piece is counted (later pieces hold larger positions), so every piece is
-// emitted and dropped before the next one is split.  After the last piece k_dd_weights reads every entry's weight:
+// emitted and dropped before the next one is split.  After the last piece k_dd_weights<false> reads every entry's weight:
 // the slot's count, or 1 for an entry without a slot.
+// bpe_load_chunks_weighted_dedup merges entries that are already weighted (the ranks' streams, back to back) the same way,
+// in one pass over one buffer: k_dd_count<true> adds the entry's weight instead of 1, and k_dd_weights<true> gives an entry
+// without a slot its own weight instead of 1.  The weights are the kernels' last parameters, which the <false>
+// instantiations do not read.
 #pragma once
 #include "common.cuh"
 
@@ -38,50 +42,58 @@ __device__ __forceinline__ u64 dd_key(const unsigned char *b, u32 len, u32 (&kw)
     return h;
 }
 
+// the slot of a chunk of len <= DD_KEY_MAX bytes, claimed if it is new (exact byte compare; a slot's key is published
+// before its tag, so nobody compares against a half-written key); adds `add` to the slot's count and atomicMin's `pos`
+// (= base + off) into its first position.  DD_NONE when no slot with these bytes or free was found within DD_PROBES probes.
+__device__ __forceinline__ u32 dd_count_one(const unsigned char *b, u32 len, DdTable T, ull add, u64 base, u64 off) {
+    u32 kw[DD_KW];
+    const u64 h = dd_key(b, len, kw);
+    const u32 tag = (u32)(h >> 32) | 2u;
+    u64 slot = h & T.mask;
+#pragma unroll 1
+    for (int probe = 0; probe < DD_PROBES; ++probe) {
+        DdSlot *S = &T.s[slot];
+        u32 t = ld_volatile_u32(&S->tag);
+        if (t == DD_EMPTY) {
+            const u32 old = atomicCAS(&S->tag, DD_EMPTY, DD_BUSY);
+            if (old == DD_EMPTY) {        // claimed: key first, then the tag that makes it visible
+                S->len = len;
+#pragma unroll
+                for (int i = 0; i < DD_KW; ++i) S->key[i] = kw[i];
+                S->first = ~0ull;
+                __threadfence();
+                atomicCAS(&S->tag, DD_BUSY, tag);   // only the claimer holds DD_BUSY
+                atomicAdd(T.used, 1ull);
+                t = tag;
+            } else {
+                t = old;
+            }
+        }
+        while (t == DD_BUSY) t = ld_volatile_u32(&S->tag);
+        __threadfence();
+        bool same = t == tag && ld_volatile_u32(&S->len) == len;
+        for (int i = 0; same && i < DD_KW; ++i) same = ld_volatile_u32(&S->key[i]) == kw[i];
+        if (same) {                       // equal tags with different bytes keep probing
+            atomicAdd(&S->count, add);
+            atomicMin(&S->first, (ull)(base + off));
+            return (u32)slot;
+        }
+        slot = (slot + 1) & T.mask;
+    }
+    return DD_NONE;
+}
+
+// WEIGHTED (bpe_load_chunks_weighted_dedup): the chunks are weighted entries, w[j] is added instead of 1 (text_pos is 0,
+// so an entry's position is its byte offset and a slot's first position is its smallest-index entry)
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(256) k_dd_count(const unsigned char *__restrict__ text, u64 m, const u64 *__restrict__ offs,
-                                                  u64 k, u64 text_pos, DdTable T, u32 *__restrict__ slot_of) {
+                                                  u64 k, u64 text_pos, DdTable T, u32 *__restrict__ slot_of,
+                                                  const u64 *__restrict__ w) {
     for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < k; j += (u64)gridDim.x * blockDim.x) {
         const u64 start = offs[j], end = j + 1 < k ? offs[j + 1] : m;
         const u64 len = end - start;
-        u32 res = DD_NONE;
-        if (len <= DD_KEY_MAX) {
-            u32 kw[DD_KW];
-            const u64 h = dd_key(text + start, (u32)len, kw);
-            const u32 tag = (u32)(h >> 32) | 2u;
-            u64 slot = h & T.mask;
-#pragma unroll 1
-            for (int probe = 0; probe < DD_PROBES; ++probe) {
-                DdSlot *S = &T.s[slot];
-                u32 t = ld_volatile_u32(&S->tag);
-                if (t == DD_EMPTY) {
-                    const u32 old = atomicCAS(&S->tag, DD_EMPTY, DD_BUSY);
-                    if (old == DD_EMPTY) {        // claimed: key first, then the tag that makes it visible
-                        S->len = (u32)len;
-#pragma unroll
-                        for (int i = 0; i < DD_KW; ++i) S->key[i] = kw[i];
-                        S->first = ~0ull;
-                        __threadfence();
-                        atomicCAS(&S->tag, DD_BUSY, tag);   // only the claimer holds DD_BUSY
-                        atomicAdd(T.used, 1ull);
-                        t = tag;
-                    } else {
-                        t = old;
-                    }
-                }
-                while (t == DD_BUSY) t = ld_volatile_u32(&S->tag);
-                __threadfence();
-                bool same = t == tag && ld_volatile_u32(&S->len) == (u32)len;
-                for (int i = 0; same && i < DD_KW; ++i) same = ld_volatile_u32(&S->key[i]) == kw[i];
-                if (same) {                       // equal tags with different bytes keep probing
-                    atomicAdd(&S->count, 1ull);
-                    atomicMin(&S->first, (ull)(text_pos + start));
-                    res = (u32)slot;
-                    break;
-                }
-                slot = (slot + 1) & T.mask;
-            }
-        }
-        slot_of[j] = res;
+        const ull add = WEIGHTED ? (ull)w[j] : 1ull;
+        slot_of[j] = len <= DD_KEY_MAX ? dd_count_one(text + start, (u32)len, T, add, text_pos, start) : DD_NONE;
     }
 }
 
@@ -142,13 +154,16 @@ __global__ void __launch_bounds__(256) k_dd_emit(const unsigned char *__restrict
     }
 }
 
-// weights of the entries: the slot's count, 1 without a slot; stats[0] += entries that have a slot
+// weights of the entries: the slot's count, 1 without a slot; stats[0] += entries that have a slot.  WEIGHTED: an entry
+// without a slot keeps its own weight w_in[idx[e]] (idx = the kept entries' input indices)
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(256) k_dd_weights(const u32 *__restrict__ slot, u64 n, DdTable T, u64 *__restrict__ wts,
-                                                    ull *__restrict__ from_table) {
+                                                    ull *__restrict__ from_table, const u64 *__restrict__ idx,
+                                                    const u64 *__restrict__ w_in) {
     u32 mine = 0;
     for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x) {
         const u32 s = slot[e];
-        wts[e] = s == DD_NONE ? 1ull : T.s[s].count;
+        wts[e] = s == DD_NONE ? (WEIGHTED ? w_in[idx[e]] : 1ull) : T.s[s].count;
         mine += s != DD_NONE;
     }
     if (mine) atomicAdd(from_table, (ull)mine);

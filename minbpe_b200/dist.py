@@ -16,6 +16,7 @@ identical copy of the global pair-count table; per merge iteration the ranks exc
 (include/b200bpe.h "step-wise training").  Tests drive the same class over gloo with a CPU
 stand-in engine built on the oracle (tests/test_dist_gloo.py).
 """
+import hashlib
 import os
 
 import numpy as np
@@ -52,10 +53,12 @@ def first_safe_cut(window):
     return int(hit[0]) + 1 if hit.size else -1
 
 
-def shard_byte_range(n_bytes, rank, world, fetch, window=1 << 20):
+def shard_byte_range(n_bytes, rank, world, fetch, window=1 << 20, empty_tail=False):
     """Byte range [lo, hi) of rank `rank`: the r-th of `world` equal parts of the text, both ends moved forward to
     the next provable chunk boundary (first_safe_cut).  fetch(lo, hi) returns the text bytes [lo, hi) as uint8
-    (a slice of an mmap, a generated block, ...).  Rank order = text order."""
+    (a slice of an mmap, a generated block, ...).  Rank order = text order.  empty_tail=True: a cut with no boundary
+    between it and the end of the text moves to the end of the text (the end is a boundary too), so the ranks after it get
+    empty ranges instead of a ValueError; for callers that handle an empty range (count_file_shard)."""
     def cut(r):
         if r <= 0:
             return 0
@@ -63,6 +66,8 @@ def shard_byte_range(n_bytes, rank, world, fetch, window=1 << 20):
             return n_bytes
         lo = n_bytes * r // world
         p = first_safe_cut(fetch(lo, min(n_bytes, lo + window)))
+        if p < 0 and empty_tail and lo + window >= n_bytes:
+            return n_bytes
         if p < 0:
             raise ValueError(f"no letter+space cut point in the {window} bytes after offset {lo}: cannot shard this text")
         return lo + p
@@ -271,6 +276,65 @@ def train_file(engine, device, path, num_merges, first_idx=256, group=None, poll
     tr.prepare(num_merges, first_idx)
     tr.run()
     return tr.result()
+
+
+def count_file_shard(engine, path, rank, world):
+    """The distinct chunks of rank `rank`'s byte range of a text file (shard_byte_range), counted on this rank's GPU
+    (Engine.load_text_gpt4_dedup, the engine's split pattern) and read back: -> (entry bytes uint8, entry offsets uint64,
+    weights uint64, chunks of the range).  The entries obey DESIGN.md §14's rule for the range; an empty range gives empty
+    arrays.  Needs no process group: a test can play every rank in one process."""
+    size = os.path.getsize(path)
+    mm = np.memmap(path, dtype=np.uint8, mode="r") if size else np.zeros(0, dtype=np.uint8)
+    lo, hi = shard_byte_range(size, rank, world, lambda a, b: mm[a:b], empty_tail=True)
+    if hi <= lo:
+        return np.zeros(0, np.uint8), np.zeros(0, np.uint64), np.zeros(0, np.uint64), 0
+    chunks, _ = engine.load_text_gpt4_dedup(mm[lo:hi])
+    del mm
+    data, offsets = engine.chunk_entries()
+    return data, offsets, engine.chunk_weights(), int(chunks)
+
+
+def load_merged_shards(engine, parts):
+    """Concatenate the ranks' count_file_shard results in rank order (= text order), rebase the offsets and merge the
+    entries of equal bytes on the GPU (Engine.load_chunks_weighted_dedup): the weighted stream of the whole file is then
+    loaded.  -> entries kept."""
+    datas = [np.asarray(p[0], dtype=np.uint8) for p in parts]
+    base = np.cumsum([0] + [d.size for d in datas[:-1]], dtype=np.uint64)
+    offsets = np.concatenate([np.asarray(p[1], dtype=np.uint64) + b for p, b in zip(parts, base)] or [np.zeros(0, np.uint64)])
+    weights = np.concatenate([np.asarray(p[2], dtype=np.uint64) for p in parts] or [np.zeros(0, np.uint64)])
+    data = np.concatenate(datas) if datas else np.zeros(0, np.uint8)
+    return engine.load_chunks_weighted_dedup(data, offsets, weights)
+
+
+def _run_digest(pairs, counts, done):
+    h = hashlib.sha256(np.ascontiguousarray(pairs, dtype=np.int32).tobytes() + np.ascontiguousarray(counts, dtype=np.int64).tobytes()
+                       + int(done).to_bytes(8, "little"))
+    return int.from_bytes(h.digest()[:8], "little") & ((1 << 63) - 1)
+
+
+def train_file_dedup(engine, path, num_merges, first_idx=256, group=None):
+    """regex.py:36-66 for a text FILE on every rank of a process group, trained on its distinct chunks: every rank counts
+    the distinct chunks of its byte range (count_file_shard), the ranks exchange their entries once (one all-gather), every
+    rank merges them into the weighted stream of the whole file on its GPU (load_merged_shards) and runs the weighted loop
+    there.  No exchange per merge.  Afterwards the ranks compare a 63-bit digest of their merges and counts (all-reduce MIN
+    and MAX) and raise RuntimeError if they differ.  Works over gloo and NCCL groups.  Returns (pairs, counts, n_done),
+    identical on every rank."""
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    part = count_file_shard(engine, path, rank, world)
+    parts = [None] * world
+    dist.all_gather_object(parts, part, group=group)
+    load_merged_shards(engine, parts)
+    del parts, part
+    pairs, counts, done = engine.train(num_merges, first_idx)
+    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
+    d = _run_digest(pairs, counts, done)
+    lo = torch.tensor([d], dtype=torch.int64, device=dev)
+    hi = lo.clone()
+    dist.all_reduce(lo, op=dist.ReduceOp.MIN, group=group)
+    dist.all_reduce(hi, op=dist.ReduceOp.MAX, group=group)
+    if int(lo.item()) != d or int(hi.item()) != d:
+        raise RuntimeError(f"train_file_dedup: rank {rank} trained different merges than another rank")
+    return pairs, counts, done
 
 
 def encode_sharded(engine, data, offsets, merges, byte_perm=None, group=None, gather=False, rank=None, world=None):

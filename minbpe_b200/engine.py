@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
 OPT_DEDUP_LOG2 = 11
@@ -56,6 +56,8 @@ def load_library():
         "bpe_read_chunk_weights": ([vp, vp, u64, P(u64)], ci),
         "bpe_load_text_gpt4_dedup": ([vp, vp, u64, P(u64), P(u64)], ci),
         "bpe_dedup_stats": ([vp, vp], ci),
+        "bpe_load_chunks_weighted_dedup": ([vp, vp, u64, vp, u64, vp, P(u64)], ci),
+        "bpe_read_chunk_entries": ([vp, vp, u64, vp, u64, P(u64), P(u64)], ci),
         "bpe_stream_len": ([vp, P(u64)], ci),
         "bpe_read_stream": ([vp, vp, u64, P(u64)], ci),
         "bpe_get_stats": ([vp, vp, vp, u64, P(u64)], ci),
@@ -175,6 +177,34 @@ class Engine:
         out = np.empty(max(n.value, 1), dtype=np.uint64)
         self._check(self._lib.bpe_read_chunk_weights(self._h, _ptr(out), out.size, ctypes.byref(n)), "bpe_read_chunk_weights")
         return out[: n.value]
+
+    def load_chunks_weighted_dedup(self, data, offsets, weights):
+        """load_chunks_weighted, with the entries of equal bytes merged on the GPU (bpe_load_chunks_weighted_dedup): the
+        entries of several weighted streams of consecutive parts of a text, back to back in text order, become the weighted
+        stream of the whole text.  -> entries kept."""
+        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        o, k = _as_offsets(offsets)
+        w = np.ascontiguousarray(weights, dtype=np.uint64)
+        if w.size != k:
+            raise EngineError(f"load_chunks_weighted_dedup: {w.size} weights for {k} chunks")
+        n = ctypes.c_uint64()
+        self._check(self._lib.bpe_load_chunks_weighted_dedup(self._h, _ptr(b) if b.size else None, b.size, _ptr(o), k,
+                                                             _ptr(w) if w.size else None, ctypes.byref(n)),
+                    "bpe_load_chunks_weighted_dedup")
+        return n.value
+
+    def chunk_entries(self):
+        """Entries of the loaded weighted stream before any train / replay: (their bytes back to back uint8, their start
+        offsets uint64)."""
+        nb, ne = ctypes.c_uint64(), ctypes.c_uint64()
+        rc = self._lib.bpe_read_chunk_entries(self._h, None, 0, None, 0, ctypes.byref(nb), ctypes.byref(ne))
+        if rc != ERR_CAPACITY:
+            self._check(rc, "bpe_read_chunk_entries")
+        b = np.empty(max(nb.value, 1), dtype=np.uint8)
+        o = np.empty(max(ne.value, 1), dtype=np.uint64)
+        self._check(self._lib.bpe_read_chunk_entries(self._h, _ptr(b), b.size, _ptr(o), o.size, ctypes.byref(nb), ctypes.byref(ne)),
+                    "bpe_read_chunk_entries")
+        return b[: nb.value], o[: ne.value]
 
     def stream_len(self):
         n = ctypes.c_uint64()

@@ -389,8 +389,11 @@ class RegexTokenizer(Tokenizer):
         is memory-mapped and split on the device in pieces; when torch.distributed is initialised (one process per
         GPU) every rank trains on its own byte range — cut where a letter is followed by a space, a provable chunk
         boundary of both patterns — and all ranks end with identical merges / vocab.  GPT-2 / GPT-4 split patterns only.
-        dedup=True: one GPU counts the file's distinct chunks (bpe_load_text_gpt4_dedup) and trains on them, so HBM holds
-        the distinct content rather than the file; not with a process group of more than one rank (ValueError)."""
+        dedup=True: train on the file's distinct chunks with their counts, so HBM holds the distinct content rather than
+        the file.  On one GPU it counts them there (bpe_load_text_gpt4_dedup); with a process group of more than one rank
+        every rank counts its own byte range, the ranks exchange their entries once and every rank merges them and trains
+        on its GPU (dist.train_file_dedup).  A group size that cannot be resolved without an initialised process group
+        raises ValueError."""
         assert vocab_size >= 256
         which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
         if which is None:
@@ -399,11 +402,23 @@ class RegexTokenizer(Tokenizer):
         from .engine import OPT_SPLIT_PATTERN
         if dedup:
             import torch.distributed as dist
-            if (group is not None and dist.get_world_size(group) > 1) or (dist.is_available() and dist.is_initialized()
-                                                                          and dist.get_world_size() > 1):
-                raise ValueError("train_from_file(dedup=True) runs on one GPU; sharded training does not count distinct chunks")
+            world = 1
+            if group is not None or (dist.is_available() and dist.is_initialized()):
+                try:      # before the file or the GPU is touched
+                    world = dist.get_world_size(group)
+                    if world > 1:
+                        dist.get_rank(group)
+                except (RuntimeError, ValueError) as ex:
+                    raise ValueError("train_from_file(dedup=True) on more than one rank needs an initialised "
+                                     "torch.distributed process group") from ex
             eng = self.engine
             eng.set_option(OPT_SPLIT_PATTERN, which)
+            if world > 1:
+                from .dist import train_file_dedup
+                pairs, counts, done = train_file_dedup(eng, path, vocab_size - 256, group=group)
+                self.last_timing = eng.timing()
+                self._adopt(pairs, counts, done, vocab_size - 256, verbose)
+                return
             data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) else np.zeros(0, dtype=np.uint8)
             eng.load_text_gpt4_dedup(data)
             del data
