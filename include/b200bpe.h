@@ -82,6 +82,24 @@ int bpe_load_chunks_weighted(bpe_handle *h, const uint8_t *bytes, uint64_t n, co
  * chunk table, is an entry of weight 1 of its own.  *n_chunks = chunks of the text, *n_entries = entries (either may be
  * NULL). */
 int bpe_load_text_gpt4_dedup(bpe_handle *h, const uint8_t *bytes, uint64_t n, uint64_t *n_chunks, uint64_t *n_entries);
+/* The same state from a stream of documents, over several calls (a counting session of the handle).  Every document is
+ * split on its own (no chunk spans two documents) and the documents count in call order, then in offset order.
+ *   bpe_dedup_begin     allocates and clears the chunk table (BPE_OPT_DEDUP_LOG2), records BPE_OPT_SPLIT_PATTERN and starts
+ *                       at text position 0; an unfinished session is discarded.
+ *   bpe_dedup_add_docs  the documents' UTF-8 bytes back to back, doc_offsets[j] = start of document j: doc_offsets[0] == 0,
+ *                       non-decreasing (empty documents are allowed), every offset <= n; n > 0 with n_docs == 0 is
+ *                       BPE_ERR_ARG.  Splits and counts them on the device in pieces (BPE_OPT_SPLIT_PIECE): whole documents
+ *                       while they fit, a longer document cut at letter+space points.  *n_chunks = chunks of this call (may
+ *                       be NULL).  Invalid arguments leave the session as it was; a failure while counting ends it.
+ *   bpe_dedup_finish    leaves the weighted stream of all the session's documents loaded, as bpe_load_text_gpt4_dedup does,
+ *                       fills bpe_dedup_stats (pieces summed over the session) and ends the session.
+ * Outside a session, bpe_dedup_add_docs and bpe_dedup_finish return BPE_ERR_STATE.  The session keeps its own table, entries,
+ * pattern and position: loads, training, encodes and option changes on the handle between two calls do not change its
+ * result.  bpe_load_text_gpt4_dedup(text) equals begin, add of one document, finish. */
+int bpe_dedup_begin(bpe_handle *h);
+int bpe_dedup_add_docs(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *doc_offsets, uint64_t n_docs,
+                       uint64_t *n_chunks);
+int bpe_dedup_finish(bpe_handle *h, uint64_t *n_chunks, uint64_t *n_entries);
 /* Entries built elsewhere, merged into one weighted stream on the device: the weighted streams of a text's consecutive
  * parts (e.g. each rank's bpe_load_text_gpt4_dedup of its byte range, read back with bpe_read_chunk_entries), concatenated
  * in text order.  Arguments and validation (and error codes) as bpe_load_chunks_weighted.  Every entry of <= 48 bytes finds
@@ -92,7 +110,7 @@ int bpe_load_text_gpt4_dedup(bpe_handle *h, const uint8_t *bytes, uint64_t n, ui
  * the input's bytes, offsets and weights, plus the table.  *n_entries = entries kept (may be NULL). */
 int bpe_load_chunks_weighted_dedup(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *chunk_offsets,
                                    uint64_t n_chunks, const uint64_t *weights, uint64_t *n_entries);
-/* Counters of the last bpe_load_text_gpt4_dedup or bpe_load_chunks_weighted_dedup: out[0] chunks of the text (the merge:
+/* Counters of the last bpe_load_text_gpt4_dedup, bpe_dedup_finish or bpe_load_chunks_weighted_dedup: out[0] chunks of the text (the merge:
  * the sum of the input weights), [1] entries, [2] entries from the table, [3] entries passed through (longer than 48 bytes,
  * or no room in the table), [4] bytes of the weighted stream, [5] table slots used, [6] table slots, [7] pieces (the
  * merge: 0). */

@@ -27,17 +27,19 @@
 #include "k_weighted.cuh"
 #include "k_dedup.cuh"
 
-#define BPE_ABI_VERSION 3
+#define BPE_ABI_VERSION 4
 
 struct EncState;
 struct SpecSet;
 struct GenEnc;
+struct DdSession;
 struct bpe_handle {
     int device = 0;
     EncState *enc = nullptr;          // memoised chunk encode (encode2_host.inl): rank table, memo, id pool, scratch
     bpe_handle *enc_scratch = nullptr;   // general encode path (encode_host.inl) works on its own stream buffers
     SpecSet *spec = nullptr;             // special tokens of the current encode call (special_host.inl)
     GenEnc *gen = nullptr;               // general encode path: device scratch + the rank table of the last merges seen (encode_host.inl)
+    DdSession *dd = nullptr;             // counting session of bpe_dedup_begin / _add_docs / _finish (dedup_host.inl)
     int sms = 0;
     cudaStream_t stream = nullptr;       // the stream every kernel of this handle runs on
     cudaStream_t own_stream = nullptr;   // created by bpe_create; `stream` may point at a caller's stream instead
@@ -95,7 +97,7 @@ struct bpe_handle {
     int opt_hist_kernel = 2;     // BPE_OPT_HIST_KERNEL: 2 = k_hist_dense (default), 1 = k_hist_dense_packed,
                                  // 0 = decide at the first large stream (cross-check + timing)
     int opt_dedup_log2 = 0;      // BPE_OPT_DEDUP_LOG2 (test hook): log2 slots of the chunk table of bpe_load_text_gpt4_dedup, 0 = default
-    u64 dd_stats[8] = {};        // bpe_dedup_stats of the last bpe_load_text_gpt4_dedup
+    u64 dd_stats[8] = {};        // bpe_dedup_stats of the last bpe_load_text_gpt4_dedup / bpe_dedup_finish
     int opt_split_pattern = 0;   // BPE_OPT_SPLIT_PATTERN: 0 = GPT-4 split pattern, 1 = GPT-2 (bpe_split_gpt4 / bpe_load_text_gpt4 / bpe_encode_text_gpt4*)
 
     bpe_timing tm = {};
@@ -108,6 +110,7 @@ static void xchg_release(bpe_handle *h);
 static void enc2_free(bpe_handle *h);
 static void spec_free(bpe_handle *h);
 static void gen_free(bpe_handle *h);
+static void dd_free(bpe_handle *h);
 static u64 g_split_piece_override = 0;   // BPE_OPT_SPLIT_PIECE (test hook): bytes per piece of the device splitter
 
 static int fail(bpe_handle *h, int code, const std::string &msg) {
@@ -242,6 +245,7 @@ extern "C" int bpe_destroy(bpe_handle *h) {
     enc2_free(h);
     spec_free(h);
     gen_free(h);
+    dd_free(h);
     if (h->enc_scratch) bpe_destroy(h->enc_scratch);
     if (h->split_slab) cudaFree(h->split_slab);
     if (h->ctl) cudaFree(h->ctl);

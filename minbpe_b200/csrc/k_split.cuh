@@ -8,6 +8,8 @@
 // few neighbouring bytes; the same header is pinned against the `regex` module on the CPU
 // (oracle/split_harness.cpp, tests/test_split_rules.py).  Here:
 //   k_split_classify    byte -> {class, char-start}                 (code-point class table from `regex`)
+//                       <true>: the documents of a piece spread into the split buffer with one boundary byte between
+//                       consecutive ones (bpe_dedup_add_docs, DESIGN.md §15)
 //   k_split_reduce      tile aggregates of the forward and of the backward scan
 //   k_split_scan_parts  exclusive scans of the aggregates (one block)
 //   k_split_apply       per tile: both scans in shared memory seeded with the carries, the rule per
@@ -33,13 +35,69 @@ struct GmemBytes {
     __device__ __forceinline__ u32 operator()(u64 pos) const { return p[pos]; }
 };
 
-// meta[i] = class of the character byte i belongs to | SM_START on its first byte
+// ---- documents (bpe_dedup_add_docs): nd documents of a piece, back to back in `src` (m bytes, doff[j] = start of
+// document j, doff[0] = 0, none empty), are split in one call with one boundary byte between consecutive ones.  In the
+// split buffer byte i of src sits at i + (its document's index); the boundary in front of document j at doff[j] + j - 1
+// holds DOC_GAP with class SC_B, so the WITH_B rule (split_logic.h) ends every run there and treats either side as end /
+// start of a text, as for a special-token occurrence of length 1 (k_special_meta).  The class is set by position: the
+// byte's value does not matter.
+#define DOC_GAP 0x00u
+#define DOC_SPAN 16   // consecutive bytes per thread of k_split_classify<true>: one binary search over doff, then a walk
+
+// the document of byte i of src: the last j with doff[j] <= i
+__device__ __forceinline__ u32 doc_of(const u64 *__restrict__ doff, u32 nd, u64 i) {
+    u32 lo = 0, hi = nd;
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (doff[mid] <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+// boundary bytes in front of position p of the split buffer: the number of j >= 1 with doff[j] + j - 1 < p
+__device__ __forceinline__ u32 gaps_before(const u64 *__restrict__ doff, u32 nd, u64 p) {
+    u32 lo = 0, hi = nd;          // invariant: the gaps of documents 1..lo lie before p, those of hi.. do not
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (doff[mid] + mid - 1 < p) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+__device__ __forceinline__ bool is_gap(const unsigned char *__restrict__ meta, u64 p) { return (meta[p] & SM_CLS) == SC_B; }
+// chunk start at position p of the split buffer of documents: not a boundary byte, and a flag of the rule or the first
+// byte of a document (the boundary's own one-byte chunk is dropped)
+__device__ __forceinline__ u32 doc_chunk_start(const unsigned char *__restrict__ flag, const unsigned char *__restrict__ meta, u64 p) {
+    return !is_gap(meta, p) && (flag[p] || (p > 0 && is_gap(meta, p - 1))) ? 1u : 0u;
+}
+
+// meta[i] = class of the character byte i belongs to | SM_START on its first byte.
+// DOCS: the split buffer `out` (n bytes) is filled from the documents in `src` first, and `b` is not read.  Every
+// document is classified on its own bytes, so a character never reaches into the next document.
+template <bool DOCS>
 __global__ void __launch_bounds__(256) k_split_classify(const unsigned char *__restrict__ b, u64 n,
                                                         const unsigned char *__restrict__ cls_table,
-                                                        unsigned char *__restrict__ meta) {
-    const GmemBytes B{b};
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x)
-        meta[i] = (unsigned char)spl_meta_of(B, i, n, cls_table);
+                                                        unsigned char *__restrict__ meta, const unsigned char *__restrict__ src,
+                                                        const u64 *__restrict__ doff, u32 nd, unsigned char *__restrict__ out) {
+    if constexpr (!DOCS) {
+        const GmemBytes B{b};
+        for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x)
+            meta[i] = (unsigned char)spl_meta_of(B, i, n, cls_table);
+    } else {
+        const u64 m = n - (nd - 1), stride = (u64)gridDim.x * blockDim.x;
+        for (u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x; t * DOC_SPAN < m; t += stride) {
+            const u64 lo = t * DOC_SPAN, hi = min(m, lo + DOC_SPAN);
+            u32 d = doc_of(doff, nd, lo);
+            u64 start = doff[d], next = d + 1 < nd ? doff[d + 1] : m;
+            for (u64 i = lo; i < hi; ++i) {
+                while (i >= next) { ++d; start = next; next = d + 1 < nd ? doff[d + 1] : m; }
+                out[i + d] = src[i];
+                meta[i + d] = (unsigned char)spl_meta_of(GmemBytes{src + start}, i - start, next - start, cls_table);
+            }
+        }
+        for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x + 1; j < nd; j += stride) {
+            out[doff[j] + j - 1] = DOC_GAP;
+            meta[doff[j] + j - 1] = (unsigned char)(SM_START | SC_B);
+        }
+    }
 }
 
 // ---- ordered block primitives for the (non-commutative) segmented operators ----
@@ -207,12 +265,16 @@ __global__ void __launch_bounds__(256) k_widen_marked(const unsigned char *__res
 }
 
 // ---- flag compaction: chunk offsets (3-kernel sum scan over the same tiles) ----
-__global__ void __launch_bounds__(SP_THREADS) k_flag_reduce(const unsigned char *__restrict__ flag, u64 n, u32 *__restrict__ part) {
+// DOCS: flags of a split buffer of documents (k_split_classify<true>): the chunk starts are doc_chunk_start's, and
+// k_flag_scatter<true> writes them at their positions in the documents' own bytes (the boundary bytes taken out)
+template <bool DOCS>
+__global__ void __launch_bounds__(SP_THREADS) k_flag_reduce(const unsigned char *__restrict__ flag, u64 n, u32 *__restrict__ part,
+                                                            const unsigned char *__restrict__ meta) {
     __shared__ u32 sm[SP_THREADS];
     const u64 base = (u64)blockIdx.x * SP_TILE + (u64)threadIdx.x * SP_ITEMS;
     u32 c = 0;
 #pragma unroll
-    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += flag[base + k];
+    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += DOCS ? doc_chunk_start(flag, meta, base + k) : flag[base + k];
     sm[threadIdx.x] = c;
     __syncthreads();
     for (int o = SP_THREADS / 2; o > 0; o >>= 1) { if (threadIdx.x < (u32)o) sm[threadIdx.x] += sm[threadIdx.x + o]; __syncthreads(); }
@@ -235,18 +297,28 @@ __global__ void __launch_bounds__(1024) k_flag_scan_parts(const u32 *__restrict_
 }
 
 // offs[] = text_base + position of every set flag (text_base: where this piece starts in the caller's text)
+template <bool DOCS>
 __global__ void __launch_bounds__(SP_THREADS) k_flag_scatter(const unsigned char *__restrict__ flag, u64 n, const u64 *__restrict__ excl,
-                                                             u64 *__restrict__ offs, u64 text_base) {
+                                                             u64 *__restrict__ offs, u64 text_base, const unsigned char *__restrict__ meta,
+                                                             const u64 *__restrict__ doff, u32 nd) {
     __shared__ u32 sm[SP_THREADS];
     const u32 tid = threadIdx.x;
     const u64 base = (u64)blockIdx.x * SP_TILE + (u64)tid * SP_ITEMS;
     u32 c = 0;
 #pragma unroll
-    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += flag[base + k];
+    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += DOCS ? doc_chunk_start(flag, meta, base + k) : flag[base + k];
     sm[tid] = c;
     __syncthreads();
     for (int o = 1; o < SP_THREADS; o <<= 1) { const u32 v = tid >= (u32)o ? sm[tid - o] : 0; __syncthreads(); sm[tid] += v; __syncthreads(); }
     u64 dst = excl[blockIdx.x] + (sm[tid] - c);
+    if constexpr (!DOCS) {
 #pragma unroll
-    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n && flag[base + k]) offs[dst++] = text_base + base + k;
+        for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n && flag[base + k]) offs[dst++] = text_base + base + k;
+    } else if (c) {
+        u64 gaps = gaps_before(doff, nd, base);
+        for (int k = 0; k < SP_ITEMS && base + k < n; ++k) {
+            if (is_gap(meta, base + k)) ++gaps;
+            else if (doc_chunk_start(flag, meta, base + k)) offs[dst++] = text_base + base + k - gaps;
+        }
+    }
 }

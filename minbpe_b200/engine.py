@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
 OPT_DEDUP_LOG2 = 11
@@ -55,6 +55,9 @@ def load_library():
         "bpe_load_chunks_weighted": ([vp, vp, u64, vp, u64, vp], ci),
         "bpe_read_chunk_weights": ([vp, vp, u64, P(u64)], ci),
         "bpe_load_text_gpt4_dedup": ([vp, vp, u64, P(u64), P(u64)], ci),
+        "bpe_dedup_begin": ([vp], ci),
+        "bpe_dedup_add_docs": ([vp, vp, u64, vp, u64, P(u64)], ci),
+        "bpe_dedup_finish": ([vp, P(u64), P(u64)], ci),
         "bpe_dedup_stats": ([vp, vp], ci),
         "bpe_load_chunks_weighted_dedup": ([vp, vp, u64, vp, u64, vp, P(u64)], ci),
         "bpe_read_chunk_entries": ([vp, vp, u64, vp, u64, P(u64), P(u64)], ci),
@@ -374,6 +377,29 @@ class Engine:
         nc, ne = ctypes.c_uint64(), ctypes.c_uint64()
         self._check(self._lib.bpe_load_text_gpt4_dedup(self._h, _ptr(b) if b.size else None, b.size, ctypes.byref(nc),
                                                        ctypes.byref(ne)), "bpe_load_text_gpt4_dedup")
+        return nc.value, ne.value
+
+    def dedup_begin(self):
+        """Start a counting session (bpe_dedup_begin): the chunk table is cleared and the split pattern
+        (OPT_SPLIT_PATTERN) recorded; an unfinished session is discarded."""
+        self._ensure_gpt4_tables()
+        self._check(self._lib.bpe_dedup_begin(self._h), "bpe_dedup_begin")
+
+    def dedup_add_docs(self, data, doc_offsets):
+        """Split and count documents in the session (bpe_dedup_add_docs): `data` = their utf-8 bytes back to back,
+        doc_offsets = the start of every document.  Every document is split on its own.  -> chunks of these documents."""
+        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        o = np.ascontiguousarray(doc_offsets, dtype=np.uint64)
+        n = ctypes.c_uint64()
+        self._check(self._lib.bpe_dedup_add_docs(self._h, _ptr(b) if b.size else None, b.size, _ptr(o) if o.size else None,
+                                                 o.size, ctypes.byref(n)), "bpe_dedup_add_docs")
+        return n.value
+
+    def dedup_finish(self):
+        """End the session and make the weighted stream of all its documents the current stream (bpe_dedup_finish).
+        -> (chunks of the documents, entries)."""
+        nc, ne = ctypes.c_uint64(), ctypes.c_uint64()
+        self._check(self._lib.bpe_dedup_finish(self._h, ctypes.byref(nc), ctypes.byref(ne)), "bpe_dedup_finish")
         return nc.value, ne.value
 
     def dedup_stats(self):

@@ -12,6 +12,8 @@ so callers and the reference's own tests work unchanged; the loops underneath ar
     train(dedup=True)  -> Engine.load_text_gpt4_dedup (device split + device chunk counting) for the texts the device
                           splits, else count_chunks + Engine.load_chunks_weighted; then Engine.train: the distinct
                           chunks with their counts, same merges as the whole text
+    train_from_iterator -> Engine.dedup_begin / dedup_add_docs / dedup_finish (every document split on its own and
+                          counted on the device, in batches) for the GPT-2 / GPT-4 patterns, else a host count
 
 What stays on the host, as in the reference: the regex pre-split for any other pattern and for
 short texts (third-party ``regex`` module, regex.py:41,114), special-token splitting
@@ -135,16 +137,20 @@ class Tokenizer:
             m[r, 0], m[r, 1] = pair
         return m
 
-    def _run_training(self, data, offsets, vocab_size, verbose, device_split=False, resume=False, weights=None, dedup=False):
+    def _run_training(self, data, offsets, vocab_size, verbose, device_split=False, resume=False, weights=None, dedup=False,
+                      session=False):
         """Shared by Basic/Regex: basic.py:21-49 / regex.py:37-70 minus the Python loops.  resume=True (not in the
         reference): keep the merges this tokenizer already has (e.g. from load()), replay them on the text and
         continue the same training run up to vocab_size — train(N) == train(k); save; load; train(N, resume=True).
         weights: the chunks are distinct chunks with these counts (count_chunks) and train as the whole text would;
-        device_split and dedup: the chunks are split and counted on the device."""
+        device_split and dedup: the chunks are split and counted on the device.  session: the engine's counting session
+        (Engine.dedup_begin / dedup_add_docs) holds the documents; its weighted stream is loaded here."""
         assert vocab_size >= 256
         num_merges = vocab_size - 256
         eng = self.engine
-        if weights is not None:
+        if session:
+            eng.dedup_finish()                 # the documents' distinct chunks, counted on the GPU (k_split.cuh, k_dedup.cuh)
+        elif weights is not None:
             eng.load_chunks_weighted(data, offsets, weights)
         elif device_split and dedup:
             eng.load_text_gpt4_dedup(data)     # split + distinct chunks counted on the GPU (k_dedup.cuh)
@@ -315,12 +321,23 @@ def count_chunks(data, offsets):
     -> (their bytes back to back, their start offsets uint64, their counts uint64).  Pairs never cross a chunk and equal
     chunks go through the same merges, so training on these with the counts as weights gives the merges, counts and
     tie-breaks of training on the whole text."""
+    return _counted(_count_into(Counter(), data, offsets))
+
+
+def _count_into(counts, data, offsets):
+    """Add the chunks of (bytes, chunk start offsets) to the Counter `counts` (dict order = first occurrence)."""
     offs = np.asarray(offsets, dtype=np.int64)
-    if offs.size == 0:
+    if offs.size:
+        raw = bytes(data)
+        ends = np.append(offs[1:], len(raw))
+        counts.update(map(raw.__getitem__, map(slice, offs.tolist(), ends.tolist())))
+    return counts
+
+
+def _counted(counts):
+    """A Counter of chunk bytes -> (their bytes back to back, their start offsets uint64, their counts uint64)."""
+    if not counts:
         return b"", np.zeros(0, dtype=np.uint64), np.zeros(0, dtype=np.uint64)
-    raw = bytes(data)
-    ends = np.append(offs[1:], len(raw))
-    counts = Counter(map(raw.__getitem__, map(slice, offs.tolist(), ends.tolist())))   # dict order = first occurrence
     lens = np.fromiter(map(len, counts), dtype=np.int64, count=len(counts))
     starts = np.zeros(len(counts), dtype=np.int64)
     np.cumsum(lens[:-1], out=starts[1:])
@@ -383,6 +400,48 @@ class RegexTokenizer(Tokenizer):
             return
         data, offsets = split_text(self.compiled_pattern, text)
         self._run_training(data, offsets, vocab_size, verbose, resume=resume)
+
+    # train_from_iterator hands the device the documents in batches of at least this many utf-8 bytes
+    ITERATOR_BATCH_BYTES = 64 << 20
+
+    def train_from_iterator(self, texts, vocab_size, verbose=False, *, resume=False):
+        """Train on an iterable of documents (str), not in the reference: the merges, vocab and verbose lines of the
+        reference's training loop (regex.py:49-70) on the chunks of every document split on its own, documents in
+        iteration order — no chunk spans two documents.  The training runs on the distinct chunks with their counts, as
+        train(dedup=True) does.  For the GPT-2 / GPT-4 patterns the documents are split and counted on the GPU in batches
+        of ITERATOR_BATCH_BYTES (bpe_dedup_add_docs), so the corpus never has to fit in host memory; other patterns are
+        split with `regex` and counted on the host.  A non-str item raises TypeError; resume=True as in train()."""
+        assert vocab_size >= 256
+        which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
+        if which is None:
+            counts = Counter()
+            for doc in texts:
+                if not isinstance(doc, str):
+                    raise TypeError(f"train_from_iterator takes str documents, got {type(doc).__name__}")
+                _count_into(counts, *split_text(self.compiled_pattern, doc))
+            data, offsets, weights = _counted(counts)
+            self._run_training(data, offsets, vocab_size, verbose, resume=resume, weights=weights)
+            return
+        from .engine import OPT_SPLIT_PATTERN
+        eng = self.engine
+        eng.set_option(OPT_SPLIT_PATTERN, which)
+        eng.dedup_begin()                          # the session records the pattern
+        batch, offs, size = [], [], 0
+        for doc in texts:
+            if not isinstance(doc, str):
+                raise TypeError(f"train_from_iterator takes str documents, got {type(doc).__name__}")
+            b = doc.encode("utf-8")
+            if not b:
+                continue
+            offs.append(size)
+            batch.append(b)
+            size += len(b)
+            if size >= self.ITERATOR_BATCH_BYTES:
+                eng.dedup_add_docs(b"".join(batch), offs)
+                batch, offs, size = [], [], 0
+        if batch:
+            eng.dedup_add_docs(b"".join(batch), offs)
+        self._run_training(None, None, vocab_size, verbose, resume=resume, session=True)
 
     def train_from_file(self, path, vocab_size, verbose=False, *, group=None, dedup=False):
         """train() for a UTF-8 text file of any size (not in the reference, which takes a str: regex.py:36).  The file
