@@ -197,7 +197,8 @@ extern "C" int bpe_create(int device, bpe_handle **out) {
     if (occ_same < 1) occ_same = 1;
     h->merge_grid_same = h->sms * occ_same;
     int occ_fast = 0;
-    if ((e = cudaFuncSetAttribute(k_merge_seg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES)) != cudaSuccess)
+    if ((e = cudaFuncSetAttribute(k_merge_seg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES)) != cudaSuccess ||
+        (e = cudaFuncSetAttribute(k_merge_seg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES)) != cudaSuccess)
         return bail("cudaFuncSetAttribute(k_merge_seg)", e);
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_fast, k_merge_seg<false>, MS_THREADS, MS_SMEM_BYTES);
     if (occ_fast < 1) return bail("k_merge_seg does not fit on an SM", cudaErrorLaunchOutOfResources);

@@ -16,7 +16,12 @@
 //
 // Batched pass (bpe_train's loop, SegArgs.batched, ctl->nk > 1): up to BATCH_MAX token-disjoint pairs that
 // k_select_batch proved to be the next merges are marked and compacted in the same single pass, with one delta
-// vector per member (DESIGN.md "Batched merges").
+// vector per member (DESIGN.md "Batched merges").  The segment loop is instantiated per member count NK (the kernel
+// switches once on the block-uniform ctl->nk): the members' ids live in registers and every member test is unrolled.
+//
+// Statistics delta per warp: the segment's merge starts go to a per-warp list (warp prefix of the lanes' counts), the
+// warp takes them 32 at a time, one per lane, and equal delta indices are folded across the warp with
+// __match_any_sync, so the CTA's delta cache sees one shared atomic per distinct index and round.
 #pragma once
 #include "common.cuh"
 #include "k_merge.cuh"
@@ -43,16 +48,17 @@
 #define MS_META 16                          // per stage: P0 P1 N0 N1 N2 seg count - | the segment's own edge record
 #define MS_BE (MS_BATCH + 2)                // edge records of a batch and of the segment on either side
 #define MS_DCACHE (1 << MS_DCACHE_LOG2)     // slots of the per-CTA delta cache (shared memory)
-#define MS_WARP_WORDS (MS_STAGES * MS_SW + MS_STAGES * MS_META + MS_BE * 8)
-#define MS_SMEM_BYTES (MS_WARPS * MS_WARP_WORDS * 4 + MS_WARPS * MS_STAGES * 8 + MS_DCACHE * 8 + 16 + BATCH_MAX * 8)
+#define MS_LIST (SEG_TOKENS / 2)            // merge starts of a segment: never two adjacent tokens, so at most half of them
+#define MS_WARP_WORDS (MS_STAGES * MS_SW + MS_STAGES * MS_META + MS_BE * 8 + MS_LIST)
+#define MS_SMEM_BYTES (MS_WARPS * MS_WARP_WORDS * 4 + MS_WARPS * MS_STAGES * 8 + MS_DCACHE * 8 + 16)
 #define MS_INVALID 0xffffffffu
 static_assert(SEG_TOKENS == 512, "k_merge_seg: a lane owns 4 rows x 4 tokens of a 512-token segment");
 static_assert((MS_SW * 4) % 16 == 0 && (MS_WARP_WORDS * 4) % 16 == 0, "bulk-copy destinations must stay 16-byte aligned");
 
-// delta[idx] += 1 through a CTA-private shared-memory cache: the same few neighbour ids are hit by
+// delta[idx] += cnt through a CTA-private shared-memory cache: the same few neighbour ids are hit by
 // almost every merge of a dense iteration (global same-address atomics serialise in L2); the
 // persistent CTA folds them here and flushes once at exit.
-__device__ __noinline__ void delta_cache_add(u32 *s_dkey, u32 *s_dcnt, ull *delta, u32 idx) {
+__device__ __noinline__ void delta_cache_add(u32 *s_dkey, u32 *s_dcnt, ull *delta, u32 idx, u32 cnt) {
     u32 slot = (idx * 2654435761u) >> (32 - MS_DCACHE_LOG2);
 #pragma unroll 1
     for (int probe = 0; probe < 4; ++probe) {
@@ -61,52 +67,106 @@ __device__ __noinline__ void delta_cache_add(u32 *s_dkey, u32 *s_dcnt, ull *delt
             const u32 old = atomicCAS(&s_dkey[slot], 0xffffffffu, idx);
             k = (old == 0xffffffffu) ? idx : old;
         }
-        if (k == idx) { atomicAdd(&s_dcnt[slot], 1u); return; }
+        if (k == idx) { atomicAdd(&s_dcnt[slot], cnt); return; }
         slot = (slot + 1) & (MS_DCACHE - 1);
     }
-    atomicAdd(&delta[idx], 1ull);   // cache neighbourhood full
+    atomicAdd(&delta[idx], (ull)cnt);   // cache neighbourhood full
 }
 
-// statistics delta of the merge that starts at the token at shared address `at` (rules: k_merge.cuh).
-// The words at s[-2..-1] and s[count..count+2] hold the neighbouring segments' tokens (or the sentinel).
-__device__ __noinline__ void delta_one(u32 at, u32 a, u32 b, u32 V, u32 *s_dkey, u32 *s_dcnt, ull *delta) {
-    const u32 t0 = lds32(at), tm1 = lds32o<-4>(at), tm2 = lds32o<-8>(at), tp2 = lds32o<8>(at), tp3 = lds32o<12>(at);
-    const bool m_m2 = (((tm2 ^ a) & TOK_MASK) == 0) && tm1 == b;   // a merge starts two tokens earlier
-    const bool m_p2 = (((tp2 ^ a) & TOK_MASK) == 0) && tp3 == b;   // a merge starts two tokens later
-    if (tm1 != TOK_SENTINEL && !(t0 & TOK_FLAG) && !m_m2) delta_cache_add(s_dkey, s_dcnt, delta, tm1 & TOK_MASK);
-    if (!(tp2 & TOK_FLAG))   // also false for the sentinel (end of stream)
-        delta_cache_add(s_dkey, s_dcnt, delta, m_p2 ? 2u * V : V + tp2);
-}
+// The members of a pass: member j is the pair (a[j], b[j]) -> z + j.  NK = 1: the one pair (a, b) -> z.  The 2·NK ids
+// are all distinct (k_select_batch), so a token is the left token of at most one member.
+template <int NK>
+struct Members {
+    u32 a[NK], b[NK];
+};
 
-// ---- batched pass (ctl->nk > 1 members, k_select_batch): the members' pairs are in shared memory at mem_a,
-//      {a_j, b_j} at byte 8j.  Their ids are all distinct, so a token is the left token of at most one member. ----
-// the member whose left id is `tok` (nk: none)
-__device__ __forceinline__ u32 batch_member(u32 tok, u32 nk, u32 mem_a) {
-    u32 j = 0;
-#pragma unroll 1
-    for (; j < nk; ++j) if (lds32(mem_a + 8 * j) == (tok & TOK_MASK)) break;
+// the member whose left id is id(x) (NK: none); bj = its right id
+template <int NK>
+__device__ __forceinline__ u32 member_of(const Members<NK> &M, u32 x, u32 &bj) {
+    u32 j = NK;
+    bj = 0;
+#pragma unroll
+    for (int k = 0; k < NK; ++k)
+        if ((x & TOK_MASK) == M.a[k]) { j = k; bj = M.b[k]; }
     return j;
 }
-// the member that starts at the token pair (t, nx) (nk: none)
-__device__ __forceinline__ u32 batch_start(u32 t, u32 nx, u32 nk, u32 mem_a) {
-    const u32 j = batch_member(t, nk, mem_a);
-    return (j < nk && lds32(mem_a + 8 * j + 4) == nx) ? j : nk;
+// a merge starts at the token pair (x, y).  NK > 1: the right id of the member whose left id is id(x) is selected, then
+// compared once (0x7fffffff: no member; no token word holds it, the sentinel carries the flag)
+template <int NK>
+__device__ __forceinline__ bool starts(const Members<NK> &M, u32 x, u32 y) {
+    if constexpr (NK == 1) {
+        return ((x ^ M.a[0]) & TOK_MASK) == 0 && y == M.b[0];
+    } else {
+        x &= TOK_MASK;
+        u32 r = TOK_MASK;
+#pragma unroll
+        for (int k = 0; k < NK; ++k) r = x == M.a[k] ? M.b[k] : r;
+        return y == r;
+    }
+}
+// the member that starts at the token pair (x, y) (NK: none)
+template <int NK>
+__device__ __forceinline__ u32 start_of(const Members<NK> &M, u32 x, u32 y) {
+    u32 bj;
+    const u32 j = member_of(M, x, bj);
+    return (j < NK && y == bj) ? j : NK;
 }
 
-// statistics delta of the merge of member j that starts at shared address `at`.  Member j is applied to the stream as
-// the members before it have left it: a neighbour that starts a merge of an earlier member m is z+m by then, one that
-// starts a merge of a later member is still itself.  Delta vector of member j: [j(2V+1), (j+1)(2V+1)), laid out as for
-// one merge.
-__device__ __noinline__ void delta_batch(u32 at, u32 nk, u32 mem_a, u32 z, u32 V, u32 *s_dkey, u32 *s_dcnt, ull *delta) {
+// statistics delta of the merge that starts at the token at shared address `at` (rules: k_merge.cuh), as the two delta
+// indices it adds 1 to (MS_INVALID: none).  The words at s[-2..-1] and s[count..count+2] hold the neighbouring segments'
+// tokens (or the sentinel).  Member j is applied to the stream as the members before it have left it: a neighbour that
+// starts a merge of an earlier member m is z+m by then, one that starts a merge of a later member is still itself.
+// Delta vector of member j: [j(2V+1), (j+1)(2V+1)), laid out as for one merge.
+template <int NK>
+__device__ __forceinline__ void start_delta(u32 at, const Members<NK> &M, u32 z, u32 V, u32 &li, u32 &ri) {
     const u32 t0 = lds32(at), tm1 = lds32o<-4>(at), tm2 = lds32o<-8>(at), tp2 = lds32o<8>(at), tp3 = lds32o<12>(at);
-    const u32 j = batch_member(t0, nk, mem_a);
-    const u32 ml = batch_start(tm2, tm1, nk, mem_a);   // member starting two tokens earlier
-    const u32 mr = batch_start(tp2, tp3, nk, mem_a);   // member starting two tokens later
+    u32 bj;
+    const u32 j = NK == 1 ? 0u : member_of(M, t0, bj);
+    const u32 ml = start_of(M, tm2, tm1);   // member starting two tokens earlier
+    const u32 mr = start_of(M, tp2, tp3);   // member starting two tokens later
     const u32 base = j * (2u * V + 1u);
-    if (tm1 != TOK_SENTINEL && !(t0 & TOK_FLAG) && ml != j)
-        delta_cache_add(s_dkey, s_dcnt, delta, base + (ml < j ? z + ml : tm1 & TOK_MASK));
-    if (!(tp2 & TOK_FLAG))
-        delta_cache_add(s_dkey, s_dcnt, delta, base + (mr == j ? 2u * V : V + (mr < j ? z + mr : tp2)));
+    li = (tm1 != TOK_SENTINEL && !(t0 & TOK_FLAG) && ml != j) ? base + (ml < j ? z + ml : tm1 & TOK_MASK) : MS_INVALID;
+    ri = !(tp2 & TOK_FLAG)   // also false for the sentinel (end of stream)
+             ? base + (mr == j ? 2u * V : V + (mr < j ? z + mr : tp2)) : MS_INVALID;
+}
+
+// one delta index per lane (MS_INVALID: none), added to the cache once per distinct index: the lowest lane of each
+// group of equal indices adds the group's size
+__device__ __forceinline__ void delta_fold_add(u32 idx, u32 lane, u32 *s_dkey, u32 *s_dcnt, ull *delta) {
+    const u32 grp = __match_any_sync(0xffffffffu, idx);
+    if (idx != MS_INVALID && lane == (u32)(__ffs(grp) - 1)) delta_cache_add(s_dkey, s_dcnt, delta, idx, (u32)__popc(grp));
+}
+
+// statistics delta of a segment's merge starts, per warp.  mall: this lane's starts, bit 4r+i = token 4·lane+i of row r.
+// The list holds the starts' byte offsets from the segment's token 0, in lane order.
+template <int NK>
+__device__ __forceinline__ void segment_delta(u32 s_a, u32 list_a, u32 lane, u32 mall, const Members<NK> &M, u32 z, u32 V,
+                                              u32 *s_dkey, u32 *s_dcnt, ull *delta) {
+    const u32 own = __popc(mall);
+    u32 incl = own;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const u32 v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= (u32)o) incl += v;
+    }
+    const u32 total = __shfl_sync(0xffffffffu, incl, 31);
+    u32 p = list_a + (incl - own) * 4u;
+#pragma unroll 1
+    while (mall) {
+        const u32 bit = __ffs(mall) - 1;
+        mall &= mall - 1;
+        sts32(p, (bit >> 2) * 512u + lane * 16u + (bit & 3u) * 4u);
+        p += 4u;
+    }
+    __syncwarp();
+#pragma unroll 1
+    for (u32 base = 0; base < total; base += 32u) {   // warp-uniform
+        u32 li = MS_INVALID, ri = MS_INVALID;
+        if (base + lane < total) start_delta(s_a + lds32(list_a + (base + lane) * 4u), M, z, V, li, ri);
+        delta_fold_add(li, lane, s_dkey, s_dcnt, delta);
+        delta_fold_add(ri, lane, s_dkey, s_dcnt, delta);
+    }
+    __syncwarp();   // the list is rewritten by the next segment
 }
 
 struct SegArgs {
@@ -122,23 +182,18 @@ struct SegArgs {
 };
 
 // one row (128 tokens, 4 per lane): merge starts m, kept tokens, replaced tokens written back to t[].
-// BATCH: the nk members at mem_a instead of (a, b) -> z; member j becomes z + j.
-template <int R, bool BATCH>
-__device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, u32 a, u32 b, u32 z, u32 nk, u32 mem_a, u32 (&t)[4],
-                                         u32 &mn, u32 &keep, u32 &dirty) {
+// Member j of M becomes z + j.  up: in, lane 31's starts of the row before (bit 3: at its last token); out, this row's.
+template <int R, int NK>
+__device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, const Members<NK> &M, u32 z, u32 (&t)[4],
+                                         u32 &mn, u32 &keep, u32 &dirty, u32 &up) {
     const uint4 q = lds128o<R * 512>(la);
-    const u32 nx = lds32o<R * 512 + 16>(la), pv = lds32o<R * 512 - 4>(la);
+    const u32 nx = lds32o<R * 512 + 16>(la);
     t[0] = q.x; t[1] = q.y; t[2] = q.z; t[3] = q.w;
-    u32 m = 0, pm = 0;
-#pragma unroll 1
-    for (u32 j = 0; j < (BATCH ? nk : 1u); ++j) {
-        if (BATCH) { a = lds32(mem_a + 8 * j); b = lds32(mem_a + 8 * j + 4); }
-        m |= (((t[0] ^ a) & TOK_MASK) == 0 && t[1] == b) ? 1u : 0u;
-        m |= (((t[1] ^ a) & TOK_MASK) == 0 && t[2] == b) ? 2u : 0u;
-        m |= (((t[2] ^ a) & TOK_MASK) == 0 && t[3] == b) ? 4u : 0u;
-        m |= (((t[3] ^ a) & TOK_MASK) == 0 && nx == b) ? 8u : 0u;
-        pm |= (((pv ^ a) & TOK_MASK) == 0 && t[0] == b) ? 1u : 0u;
-    }
+    const u32 m = (starts(M, t[0], t[1]) ? 1u : 0u) | (starts(M, t[1], t[2]) ? 2u : 0u) | (starts(M, t[2], t[3]) ? 4u : 0u) |
+                  (starts(M, t[3], nx) ? 8u : 0u);
+    // a start at the token in front of this lane's first one: the lane before tested that pair (lane 0: lane 31, row before)
+    const u32 pm = __shfl_sync(0xffffffffu, lane == 31 ? up : m, (lane + 31) & 31) >> 3;
+    up = m;
     const u32 d = ((m << 1) | pm) & 0xfu;   // dropped: the token after a merge start
     u32 valid = 0xfu;
     if (R * 128u + 128u > count) {          // warp-uniform: the row that holds the end of the segment
@@ -149,7 +204,12 @@ __device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, u32 a, u32
     keep = ~d & valid;
     dirty |= (mn | (keep ^ valid)) ? (1u << R) : 0u;
     if (mn) {                               // few lanes: the merged token takes its place in the registers
-        auto zof = [&](u32 x) { return (BATCH ? z + batch_member(x, nk, mem_a) : z) | (x & TOK_FLAG); };
+        auto zof = [&](u32 x) {
+            u32 id = z;
+#pragma unroll
+            for (int j = 1; j < NK; ++j) if ((x & TOK_MASK) == M.a[j]) id = z + j;
+            return id | (x & TOK_FLAG);
+        };
         if (mn & 1u) t[0] = zof(t[0]);
         if (mn & 2u) t[1] = zof(t[1]);
         if (mn & 4u) t[2] = zof(t[2]);
@@ -175,21 +235,16 @@ __device__ __forceinline__ void scatter_row(u32 s_a, u32 lane, u32 off, u32 row_
     }
 }
 
-// LIST = false: every segment of the stream, MS_BATCH consecutive ones per ticket.  LIST = true: only the candidate segments
-// k_seg_filter put on the list at ctl->cand_ptr, one per ticket (the filter carried the other segments' edge records over).
-template <bool LIST>
-__global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs A) {
+// The pass over the segments with NK members (k_merge_seg below picks NK).
+template <bool LIST, int NK>
+__device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
     Ctl *ctl = A.ctl;
-    if (!A.force && (ctl->done || ctl->overflow || ctl->iter >= ctl->max_iter)) return;
-    if (ctl->a == ctl->b) return;  // pairs (a,a) take the pack + k_merge<true> path
-
     extern __shared__ __align__(128) unsigned char smem_raw[];
     u32 *s_warp = reinterpret_cast<u32 *>(smem_raw);                              // [MS_WARPS][MS_WARP_WORDS]
     u64 *s_bar = reinterpret_cast<u64 *>(s_warp + MS_WARPS * MS_WARP_WORDS);      // [MS_WARPS][MS_STAGES]
     u32 *s_dkey = reinterpret_cast<u32 *>(s_bar + MS_WARPS * MS_STAGES);          // [MS_DCACHE] delta index or 0xffffffff
     u32 *s_dcnt = s_dkey + MS_DCACHE;                                             // [MS_DCACHE]
     ull *s_drops = reinterpret_cast<ull *>(s_dcnt + MS_DCACHE);
-    u32 *s_mem = reinterpret_cast<u32 *>(s_drops + 1);                            // [BATCH_MAX][2] members of a batched pass
 
     const u32 FULL = 0xffffffffu;
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -197,10 +252,14 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
     u32 *__restrict__ w = ctl->cur ? A.buf1 : A.buf0;                 // compacted in place
     const Edge *__restrict__ e_cur = ctl->edge_cur ? A.e1 : A.e0;
     Edge *__restrict__ e_next = ctl->edge_cur ? A.e0 : A.e1;
-    const u32 a = (u32)ctl->a, b = (u32)ctl->b, z = (u32)ctl->z;
+    const u32 z = (u32)ctl->z;
     const u32 nseg = ctl->nseg;
-    const u32 nk = (!LIST && A.batched) ? ctl->nk : 1u;   // block-uniform
-    const u32 mem_a = smem_addr(s_mem);
+    Members<NK> M;
+#pragma unroll
+    for (int j = 0; j < NK; ++j) {
+        M.a[j] = j ? (u32)ctl->bat_a[j] : (u32)ctl->a;
+        M.b[j] = j ? (u32)ctl->bat_b[j] : (u32)ctl->b;
+    }
     ull *const delta = A.xbase ? x_local_delta(A.xbase, A.xstride) : A.delta;
     const u32 *__restrict__ cand = LIST ? reinterpret_cast<const u32 *>(ctl->cand_ptr) : nullptr;
     const u32 n_cand = LIST ? ctl->n_cand : 0u;
@@ -209,6 +268,7 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
     const u32 ws_a = smem_addr(s_warp + warp * MS_WARP_WORDS);   // [MS_STAGES][MS_SW] staging ring
     const u32 wmeta_a = ws_a + MS_STAGES * MS_SW * 4;            // [MS_STAGES][MS_META]
     const u32 wbe_a = wmeta_a + MS_STAGES * MS_META * 4;         // [MS_BE][8] edge records batch_seg-1 .. batch_seg+MS_BATCH
+    const u32 wlist_a = wbe_a + MS_BE * 32;                      // [MS_LIST] merge starts of the segment (segment_delta)
     const u32 wbar_a = smem_addr(s_bar + warp * MS_STAGES);
 
     if (lane == 0) {
@@ -217,7 +277,6 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
     }
     for (u32 i = tid; i < MS_DCACHE; i += MS_THREADS) { s_dkey[i] = 0xffffffffu; s_dcnt[i] = 0; }
     if (tid == 0) *s_drops = 0;
-    if (tid < nk) { s_mem[2 * tid] = tid ? (u32)ctl->bat_a[tid] : a; s_mem[2 * tid + 1] = tid ? (u32)ctl->bat_b[tid] : b; }
     __syncthreads();
 
     // ---- issue side: next non-empty segment of this warp -> bulk copy into `stage` ----
@@ -321,17 +380,11 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
         u32 t[4][4], mn[4] = {0, 0, 0, 0}, keep[4] = {0, 0, 0, 0};
         u32 dirty = 0;
         const u32 la = s_a + lane * 16;
-        if (nk == 1u) {
-            mark_row<0, false>(la, lane, count, a, b, z, 1u, mem_a, t[0], mn[0], keep[0], dirty);
-            if (count > 128u) mark_row<1, false>(la, lane, count, a, b, z, 1u, mem_a, t[1], mn[1], keep[1], dirty);
-            if (count > 256u) mark_row<2, false>(la, lane, count, a, b, z, 1u, mem_a, t[2], mn[2], keep[2], dirty);
-            if (count > 384u) mark_row<3, false>(la, lane, count, a, b, z, 1u, mem_a, t[3], mn[3], keep[3], dirty);
-        } else {
-            mark_row<0, true>(la, lane, count, a, b, z, nk, mem_a, t[0], mn[0], keep[0], dirty);
-            if (count > 128u) mark_row<1, true>(la, lane, count, a, b, z, nk, mem_a, t[1], mn[1], keep[1], dirty);
-            if (count > 256u) mark_row<2, true>(la, lane, count, a, b, z, nk, mem_a, t[2], mn[2], keep[2], dirty);
-            if (count > 384u) mark_row<3, true>(la, lane, count, a, b, z, nk, mem_a, t[3], mn[3], keep[3], dirty);
-        }
+        u32 up = starts(M, lds32o<-4>(s_a), lds32(s_a)) ? 8u : 0u;   // the pair (s[-1], s[0]), as lane 31 of row -1
+        mark_row<0>(la, lane, count, M, z, t[0], mn[0], keep[0], dirty, up);
+        if (count > 128u) mark_row<1>(la, lane, count, M, z, t[1], mn[1], keep[1], dirty, up);
+        if (count > 256u) mark_row<2>(la, lane, count, M, z, t[2], mn[2], keep[2], dirty, up);
+        if (count > 384u) mark_row<3>(la, lane, count, M, z, t[3], mn[3], keep[3], dirty, up);
         dirty = __reduce_or_sync(FULL, dirty);   // rows in which some token is replaced or dropped
         if (!dirty) {
             // untouched segment: nothing to write, the edge record carries over
@@ -341,17 +394,8 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
         }
 
         // ---- statistics delta of this segment's merge starts (reads the stage before it is rewritten) ----
-        if (delta) {
-            u32 mall = mn[0] | (mn[1] << 4) | (mn[2] << 8) | (mn[3] << 12);
-#pragma unroll 1
-            while (mall) {   // one pass per merge start of this lane
-                const int bit = __ffs(mall) - 1;
-                mall &= mall - 1;
-                const u32 at = la + (bit >> 2) * 512 + (bit & 3) * 4;
-                if (nk == 1u) delta_one(at, a, b, A.V, s_dkey, s_dcnt, delta);
-                else delta_batch(at, nk, mem_a, z, A.V, s_dkey, s_dcnt, delta);
-            }
-        }
+        if (delta)
+            segment_delta(s_a, wlist_a, lane, mn[0] | (mn[1] << 4) | (mn[2] << 8) | (mn[3] << 12), M, z, A.V, s_dkey, s_dcnt, delta);
 
         // ---- kept tokens per lane and row, packed one byte per row: one warp scan for all four rows ----
         const u32 own = __popc(keep[0]) | (__popc(keep[1]) << 8) | (__popc(keep[2]) << 16) | (__popc(keep[3]) << 24);
@@ -418,9 +462,30 @@ __global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs 
             ctl->n = n - dropped;
             ctl->drops = 0;
             ctl->edge_cur ^= 1u;
-            ctl->iter += nk;
+            ctl->iter += NK;
             ctl->epoch += 1;
             ctl->merge_ticket = 0; ctl->merge_exit = 0;
+        }
+    }
+}
+
+// LIST = false: every segment of the stream, MS_BATCH consecutive ones per ticket.  LIST = true: only the candidate segments
+// k_seg_filter put on the list at ctl->cand_ptr, one per ticket (the filter carried the other segments' edge records over).
+// The segment filter and the sharded loop only ever run one member, so LIST takes the NK = 1 pass alone.
+template <bool LIST>
+__global__ void __launch_bounds__(MS_THREADS, MS_MINBLOCKS) k_merge_seg(SegArgs A) {
+    const Ctl *ctl = A.ctl;
+    if (!A.force && (ctl->done || ctl->overflow || ctl->iter >= ctl->max_iter)) return;
+    if (ctl->a == ctl->b) return;  // pairs (a,a) take the pack + k_merge<true> path
+    static_assert(BATCH_MAX == 4, "k_merge_seg: one pass per member count 1..BATCH_MAX");
+    if constexpr (LIST) {
+        merge_seg_pass<true, 1>(A);
+    } else {
+        switch (A.batched ? ctl->nk : 1u) {   // block-uniform
+        case 2: merge_seg_pass<false, 2>(A); break;
+        case 3: merge_seg_pass<false, 3>(A); break;
+        case 4: merge_seg_pass<false, 4>(A); break;
+        default: merge_seg_pass<false, 1>(A); break;
         }
     }
 }

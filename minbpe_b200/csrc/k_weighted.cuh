@@ -137,7 +137,7 @@ __device__ __forceinline__ u32 wt_member(u32 x, u32 y, u32 nk, const u32 *ma, co
     return j;
 }
 
-// Statistics delta of a merge pass with a != b on the segmented stream, weighted: the rules of delta_one / delta_batch
+// Statistics delta of a merge pass with a != b on the segmented stream, weighted: the rules of start_delta
 // (k_merge_seg.cuh) with the weight of the merge's entry in place of 1.  Runs before the merge pass, on the stream the
 // pass reads.  batched: the ctl->nk members k_select_batch chose, one delta vector of 2V+1 counters each.
 __global__ void __launch_bounds__(256) k_wt_delta_seg(const u32 *__restrict__ buf0, const u32 *__restrict__ buf1, const Ctl *ctl,
