@@ -159,6 +159,25 @@ static int alloc_table(bpe_handle *h, Table &t, u64 cap, bool with_first) {
 
 static u64 next_pow2(u64 x) { u64 p = 1; while (p < x) p <<= 1; return p; }
 
+// grow-only device buffer of `elem`-byte elements; the first `used` elements are kept
+struct DevBuf {
+    void *p = nullptr; u64 cap = 0;
+    ~DevBuf() { if (p) cudaFree(p); }
+    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
+};
+static int dev_grow(bpe_handle *h, DevBuf &b, u64 need, u64 used, size_t elem) {
+    if (need <= b.cap) return BPE_OK;
+    const u64 nc = std::max<u64>(need, b.cap * 2);
+    void *q = nullptr;
+    CU(cudaMalloc(&q, std::max<u64>(nc, 1) * elem));
+    cudaError_t e = used ? cudaMemcpyAsync(q, b.p, used * elem, cudaMemcpyDeviceToDevice, h->stream) : cudaSuccess;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) { cudaFree(q); return fail(h, BPE_ERR_CUDA, std::string("dev_grow: ") + cudaGetErrorString(e)); }
+    if (b.p) cudaFree(b.p);
+    b.p = q; b.cap = nc;
+    return BPE_OK;
+}
+
 extern "C" int bpe_create(int device, bpe_handle **out) {
     bpe_handle *h = nullptr;
     if (!out) return fail(nullptr, BPE_ERR_ARG, "bpe_create: out is NULL");
@@ -546,16 +565,29 @@ static int wt_finish(bpe_handle *h, u64 n_entries) {
     return BPE_OK;
 }
 
+// the arguments of bpe_load_chunks_weighted / bpe_load_chunks_weighted_dedup: a non-empty text tiled by its chunks, a weight
+// >= 1 per chunk, then the checks of bpe_load_stream; *wsum = the sum of the weights
+static int check_weighted(bpe_handle *h, const char *who, const uint8_t *bytes, u64 n, const uint64_t *chunk_offsets,
+                          u64 n_chunks, const uint64_t *weights, u64 *wsum) {
+    if (n && (!chunk_offsets || !n_chunks)) return fail(h, BPE_ERR_ARG, std::string(who) + ": a non-empty text needs chunk offsets");
+    if (!n && n_chunks) return fail(h, BPE_ERR_ARG, std::string(who) + ": chunks of an empty text");
+    if (n_chunks && !weights) return fail(h, BPE_ERR_ARG, "weights is NULL");
+    *wsum = 0;
+    for (u64 i = 0; i < n_chunks; ++i) {
+        if (weights[i] == 0) return fail(h, BPE_ERR_ARG, "weights must be >= 1");
+        *wsum += weights[i];
+    }
+    if (!bytes && n) return fail(h, BPE_ERR_ARG, "bytes is NULL");
+    if (n >= (1ull << 36)) return fail(h, BPE_ERR_ARG, "stream too long (limit 2^36 tokens)");
+    return check_offsets(h, chunk_offsets, n_chunks, n);
+}
+
 extern "C" int bpe_load_chunks_weighted(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *chunk_offsets,
                                         uint64_t n_chunks, const uint64_t *weights) {
     if (!h) return BPE_ERR_ARG;
-    if (n && (!chunk_offsets || !n_chunks)) return fail(h, BPE_ERR_ARG, "bpe_load_chunks_weighted: a non-empty text needs chunk offsets");
-    if (!n && n_chunks) return fail(h, BPE_ERR_ARG, "bpe_load_chunks_weighted: chunks of an empty text");
-    if (n_chunks && !weights) return fail(h, BPE_ERR_ARG, "weights is NULL");
-    for (u64 i = 0; i < n_chunks; ++i)
-        if (weights[i] == 0) return fail(h, BPE_ERR_ARG, "weights must be >= 1");
-    int rc = bpe_load_stream(h, bytes, n, chunk_offsets, n_chunks);   // validates the rest; leaves an unweighted stream
-    if (rc) return rc;
+    u64 wsum = 0;
+    int rc = check_weighted(h, "bpe_load_chunks_weighted", bytes, n, chunk_offsets, n_chunks, weights, &wsum);
+    if (rc || (rc = bpe_load_stream(h, bytes, n, chunk_offsets, n_chunks))) return rc;   // leaves an unweighted stream
     h->loaded = false;
     if ((rc = wt_alloc(h, n_chunks))) return rc;
     if (n_chunks) CU(cudaMemcpyAsync(h->wts, weights, n_chunks * 8, cudaMemcpyHostToDevice, h->stream));

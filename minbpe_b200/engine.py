@@ -106,11 +106,26 @@ def _ptr(a):
     return None if a is None else ctypes.c_void_p(a.ctypes.data)
 
 
+def _u8(data):
+    """Bytes-like object or array -> contiguous uint8 array (a view where possible)."""
+    return np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+
+
 def _as_offsets(offs):
     if offs is None:
         return None, 0
     o = np.ascontiguousarray(offs, dtype=np.uint64)
     return o, int(o.size)
+
+
+def _weighted_args(what, data, offsets, weights):
+    """-> (the arrays, the arguments after the handle) of bpe_load_chunks_weighted / bpe_load_chunks_weighted_dedup."""
+    b = _u8(data)
+    o, k = _as_offsets(offsets)
+    w = np.ascontiguousarray(weights, dtype=np.uint64)
+    if w.size != k:
+        raise EngineError(f"{what}: {w.size} weights for {k} chunks")
+    return (b, o, w), (_ptr(b) if b.size else None, b.size, _ptr(o), k, _ptr(w) if w.size else None)
 
 
 class Engine:
@@ -148,7 +163,7 @@ class Engine:
 
     # ---- corpus ----
     def load_stream(self, data, offsets=None):
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         o, k = _as_offsets(offsets)
         self._keep = (b, o)
         self._check(self._lib.bpe_load_stream(self._h, _ptr(b) if b.size else None, b.size, _ptr(o), k), "bpe_load_stream")
@@ -162,14 +177,8 @@ class Engine:
         """A weighted stream (bpe_load_chunks_weighted): entries = chunk occurrences in text order (bytes back to back,
         start offsets), weights[k] >= 1 = how many occurrences of the same bytes entry k stands for.  train() on it gives
         the merges and counts of training on the whole text."""
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
-        o, k = _as_offsets(offsets)
-        w = np.ascontiguousarray(weights, dtype=np.uint64)
-        if w.size != k:
-            raise EngineError(f"load_chunks_weighted: {w.size} weights for {k} chunks")
-        self._keep = (b, o, w)
-        self._check(self._lib.bpe_load_chunks_weighted(self._h, _ptr(b) if b.size else None, b.size, _ptr(o), k,
-                                                       _ptr(w) if w.size else None), "bpe_load_chunks_weighted")
+        self._keep, args = _weighted_args("load_chunks_weighted", data, offsets, weights)
+        self._check(self._lib.bpe_load_chunks_weighted(self._h, *args), "bpe_load_chunks_weighted")
 
     def chunk_weights(self):
         """Weights of the entries of the loaded weighted stream, in stream order (uint64)."""
@@ -185,15 +194,9 @@ class Engine:
         """load_chunks_weighted, with the entries of equal bytes merged on the GPU (bpe_load_chunks_weighted_dedup): the
         entries of several weighted streams of consecutive parts of a text, back to back in text order, become the weighted
         stream of the whole text.  -> entries kept."""
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
-        o, k = _as_offsets(offsets)
-        w = np.ascontiguousarray(weights, dtype=np.uint64)
-        if w.size != k:
-            raise EngineError(f"load_chunks_weighted_dedup: {w.size} weights for {k} chunks")
+        keep, args = _weighted_args("load_chunks_weighted_dedup", data, offsets, weights)   # args point into keep
         n = ctypes.c_uint64()
-        self._check(self._lib.bpe_load_chunks_weighted_dedup(self._h, _ptr(b) if b.size else None, b.size, _ptr(o), k,
-                                                             _ptr(w) if w.size else None, ctypes.byref(n)),
-                    "bpe_load_chunks_weighted_dedup")
+        self._check(self._lib.bpe_load_chunks_weighted_dedup(self._h, *args, ctypes.byref(n)), "bpe_load_chunks_weighted_dedup")
         return n.value
 
     def chunk_entries(self):
@@ -252,7 +255,7 @@ class Engine:
 
     def encode(self, data, offsets, merges, byte_perm=None):
         """-> ids int32.  merges: [M,2] int32 in rank order (id of rank r = 256 + r)."""
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         o, k = _as_offsets(offsets)
         m = np.ascontiguousarray(np.asarray(merges, dtype=np.int32).reshape(-1, 2))
         perm = None if byte_perm is None else np.ascontiguousarray(byte_perm, dtype=np.uint8)
@@ -293,7 +296,7 @@ class Engine:
         specials: [(utf-8 bytes, id), ...] in the order of the special_tokens dict — their occurrences are found on the
         GPU as well and every part between them is encoded on its own (regex.py:152-163)."""
         self._ensure_gpt4_tables()
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         m = np.ascontiguousarray(np.asarray(merges, dtype=np.int32).reshape(-1, 2))
         perm = None if byte_perm is None else np.ascontiguousarray(byte_perm, dtype=np.uint8)
         if out is None:
@@ -353,7 +356,7 @@ class Engine:
     def split_gpt4(self, data):
         """Chunk start offsets (uint64) of utf-8 `data` under GPT4_SPLIT_PATTERN, computed on the GPU."""
         self._ensure_gpt4_tables()
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         out = np.empty(max(b.size, 1), dtype=np.uint64)
         n = ctypes.c_uint64()
         self._check(self._lib.bpe_split_gpt4(self._h, _ptr(b) if b.size else None, b.size, _ptr(out), out.size, ctypes.byref(n)),
@@ -363,7 +366,7 @@ class Engine:
     def load_text_gpt4(self, data, count_chunks=False):
         """Upload utf-8 `data`, split it with GPT4_SPLIT_PATTERN on the GPU and make it the current stream."""
         self._ensure_gpt4_tables()
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         n = ctypes.c_uint64()
         self._check(self._lib.bpe_load_text_gpt4(self._h, _ptr(b) if b.size else None, b.size,
                                                  ctypes.byref(n) if count_chunks else None), "bpe_load_text_gpt4")
@@ -373,7 +376,7 @@ class Engine:
         """Upload utf-8 `data`, split it on the GPU (BPE_OPT_SPLIT_PATTERN), count its distinct chunks there and make the
         weighted stream of the distinct chunks with their counts the current stream.  -> (chunks of the text, entries)."""
         self._ensure_gpt4_tables()
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         nc, ne = ctypes.c_uint64(), ctypes.c_uint64()
         self._check(self._lib.bpe_load_text_gpt4_dedup(self._h, _ptr(b) if b.size else None, b.size, ctypes.byref(nc),
                                                        ctypes.byref(ne)), "bpe_load_text_gpt4_dedup")
@@ -388,7 +391,7 @@ class Engine:
     def dedup_add_docs(self, data, doc_offsets):
         """Split and count documents in the session (bpe_dedup_add_docs): `data` = their utf-8 bytes back to back,
         doc_offsets = the start of every document.  Every document is split on its own.  -> chunks of these documents."""
-        b = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        b = _u8(data)
         o = np.ascontiguousarray(doc_offsets, dtype=np.uint64)
         n = ctypes.c_uint64()
         self._check(self._lib.bpe_dedup_add_docs(self._h, _ptr(b) if b.size else None, b.size, _ptr(o) if o.size else None,

@@ -137,27 +137,15 @@ class Tokenizer:
             m[r, 0], m[r, 1] = pair
         return m
 
-    def _run_training(self, data, offsets, vocab_size, verbose, device_split=False, resume=False, weights=None, dedup=False,
-                      session=False):
-        """Shared by Basic/Regex: basic.py:21-49 / regex.py:37-70 minus the Python loops.  resume=True (not in the
-        reference): keep the merges this tokenizer already has (e.g. from load()), replay them on the text and
-        continue the same training run up to vocab_size — train(N) == train(k); save; load; train(N, resume=True).
-        weights: the chunks are distinct chunks with these counts (count_chunks) and train as the whole text would;
-        device_split and dedup: the chunks are split and counted on the device.  session: the engine's counting session
-        (Engine.dedup_begin / dedup_add_docs) holds the documents; its weighted stream is loaded here."""
+    def _run_training(self, load, vocab_size, verbose, resume=False):
+        """Shared by Basic/Regex: basic.py:21-49 / regex.py:37-70 minus the Python loops.  load() puts the training stream
+        on self.engine: the text's chunks, or its distinct chunks with their counts, which train as the whole text would.
+        resume=True (not in the reference): keep the merges this tokenizer already has (e.g. from load()), replay them on
+        the text and continue the same training run up to vocab_size — train(N) == train(k); save; load; train(N, resume=True)."""
         assert vocab_size >= 256
         num_merges = vocab_size - 256
         eng = self.engine
-        if session:
-            eng.dedup_finish()                 # the documents' distinct chunks, counted on the GPU (k_split.cuh, k_dedup.cuh)
-        elif weights is not None:
-            eng.load_chunks_weighted(data, offsets, weights)
-        elif device_split and dedup:
-            eng.load_text_gpt4_dedup(data)     # split + distinct chunks counted on the GPU (k_dedup.cuh)
-        elif device_split:
-            eng.load_text_gpt4(data)      # regex.py:41-44 on the GPU (k_split.cuh)
-        else:
-            eng.load_stream(data, offsets)
+        load()
         have = None
         if resume and self.merges:
             have = self._merge_array()
@@ -272,7 +260,8 @@ class BasicTokenizer(Tokenizer):
 
     def train(self, text, vocab_size, verbose=False, *, resume=False):
         assert vocab_size >= 256
-        self._run_training(text.encode("utf-8"), None, vocab_size, verbose, resume=resume)
+        data = text.encode("utf-8")
+        self._run_training(lambda: self.engine.load_stream(data), vocab_size, verbose, resume=resume)
 
     def decode(self, ids):
         if self._decode_on_device(len(ids)):
@@ -387,19 +376,16 @@ class RegexTokenizer(Tokenizer):
         `regex` and counted on the host (count_chunks)."""
         assert vocab_size >= 256
         data = text.encode("utf-8")
-        if dedup:
-            if self._device_split(len(data)):
-                self._run_training(data, None, vocab_size, verbose, device_split=True, resume=resume, dedup=True)
-                return
-            data, offsets = split_text(self.compiled_pattern, text)
-            data, offsets, weights = count_chunks(data, offsets)
-            self._run_training(data, offsets, vocab_size, verbose, resume=resume, weights=weights)
-            return
         if self._device_split(len(data)):
-            self._run_training(data, None, vocab_size, verbose, device_split=True, resume=resume)
+            # regex.py:41-44 on the GPU (k_split.cuh); dedup: the distinct chunks counted there too (k_dedup.cuh)
+            self._run_training(lambda: (self.engine.load_text_gpt4_dedup if dedup else self.engine.load_text_gpt4)(data),
+                               vocab_size, verbose, resume=resume)
             return
-        data, offsets = split_text(self.compiled_pattern, text)
-        self._run_training(data, offsets, vocab_size, verbose, resume=resume)
+        chunks = split_text(self.compiled_pattern, text)
+        if dedup:
+            chunks = count_chunks(*chunks)
+        self._run_training(lambda: (self.engine.load_chunks_weighted if dedup else self.engine.load_stream)(*chunks),
+                           vocab_size, verbose, resume=resume)
 
     # train_from_iterator hands the device the documents in batches of at least this many utf-8 bytes
     ITERATOR_BATCH_BYTES = 64 << 20
@@ -419,8 +405,8 @@ class RegexTokenizer(Tokenizer):
                 if not isinstance(doc, str):
                     raise TypeError(f"train_from_iterator takes str documents, got {type(doc).__name__}")
                 _count_into(counts, *split_text(self.compiled_pattern, doc))
-            data, offsets, weights = _counted(counts)
-            self._run_training(data, offsets, vocab_size, verbose, resume=resume, weights=weights)
+            chunks = _counted(counts)
+            self._run_training(lambda: self.engine.load_chunks_weighted(*chunks), vocab_size, verbose, resume=resume)
             return
         from .engine import OPT_SPLIT_PATTERN
         eng = self.engine
@@ -441,7 +427,7 @@ class RegexTokenizer(Tokenizer):
                 batch, offs, size = [], [], 0
         if batch:
             eng.dedup_add_docs(b"".join(batch), offs)
-        self._run_training(None, None, vocab_size, verbose, resume=resume, session=True)
+        self._run_training(eng.dedup_finish, vocab_size, verbose, resume=resume)
 
     def train_from_file(self, path, vocab_size, verbose=False, *, group=None, dedup=False):
         """train() for a UTF-8 text file of any size (not in the reference, which takes a str: regex.py:36).  The file
@@ -478,12 +464,10 @@ class RegexTokenizer(Tokenizer):
                 self.last_timing = eng.timing()
                 self._adopt(pairs, counts, done, vocab_size - 256, verbose)
                 return
-            data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) else np.zeros(0, dtype=np.uint8)
-            eng.load_text_gpt4_dedup(data)
-            del data
-            pairs, counts, done = eng.train(vocab_size - 256)
-            self.last_timing = eng.timing()
-            self._adopt(pairs, counts, done, vocab_size - 256, verbose)
+            def load():   # the mapping is dropped before the merge loop starts
+                data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) else np.zeros(0, dtype=np.uint8)
+                eng.load_text_gpt4_dedup(data)
+            self._run_training(load, vocab_size, verbose)
             return
         from .dist import train_file
         eng = self.engine

@@ -89,18 +89,25 @@ def test_boundaries_change_the_split():
         assert not np.array_equal(expected(docs, pat), expected(["".join(docs)], pat))
 
 
-def test_host_path_for_other_patterns(monkeypatch):
+def test_host_path_for_other_patterns_loader(monkeypatch):
     """A pattern the device does not split: every document split with `regex` on its own, the chunks counted in one host
     Counter in first-occurrence order across documents; the weighted oracle loop on them gives the merges of the plain
-    loop on the whole per-document chunk list."""
+    loop on the whole per-document chunk list.  The loader handed to _run_training is run against a stub engine that
+    records what it loads."""
     from minbpe_b200 import RegexTokenizer
     pattern = r"\p{L}+|\s+|[^\s\p{L}]+"
     rnd = random.Random(8)
     docs = ["".join(rnd.choice(ALPHABET) for _ in range(rnd.randint(0, 30))) for _ in range(400)]
     got = {}
 
-    def capture(self, data, offsets, vocab_size, verbose, **kw):
-        got.update(data=data, offsets=offsets, weights=kw["weights"], resume=kw["resume"])
+    class Loaded:     # the engine the loader puts the stream on: records what it received
+        def load_chunks_weighted(self, data, offsets, weights):
+            got.update(data=data, offsets=offsets, weights=weights)
+
+    def capture(self, load, vocab_size, verbose, resume=False):
+        load()
+        got.update(resume=resume)
+    monkeypatch.setattr(RegexTokenizer, "engine", property(lambda self: Loaded()))
     monkeypatch.setattr(RegexTokenizer, "_run_training", capture)
     RegexTokenizer(pattern).train_from_iterator(iter(docs), 300)
     chunks = [c.encode("utf-8") for d in docs for c in regex.findall(pattern, d)]
