@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
@@ -29,63 +30,106 @@
 
 #define BPE_ABI_VERSION 4
 
+namespace {   // the owner types stay private to the library: they add no exported symbol
+
+// A device allocation of `cap` elements of T with one owner: the destructor frees it, a move hands it on, a copy does not
+// compile.  It converts to T *, so kernel arguments and cudaMemcpyAsync / cudaMemsetAsync take it as they are.
+template <class T>
+struct DevBuf {
+    T *p = nullptr;
+    u64 cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        if (this != &o) { reset(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+        return *this;
+    }
+    ~DevBuf() { reset(); }
+    void reset() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    operator T *() const { return p; }
+    T *operator->() const { return p; }   // device addresses of fields (&h->ctl->n)
+};
+
+// A CUDA event with one owner (timing on the handle's stream)
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event &) = delete;
+    Event &operator=(const Event &) = delete;
+    Event(Event &&o) noexcept : e(o.e) { o.e = nullptr; }
+    ~Event() { if (e) cudaEventDestroy(e); }
+    cudaError_t create() { return cudaEventCreate(&e); }
+    operator cudaEvent_t() const { return e; }
+};
+
+// The pair-count table's device arrays; the kernels take the Table view by value
+struct PairTable {
+    DevBuf<u64> keys, counts, first;
+    u64 mask = 0;   // slots - 1
+    operator Table() const { return {keys, counts, first, mask}; }
+};
+
+}  // namespace
+
 struct EncState;
 struct SpecSet;
 struct GenEnc;
 struct DdSession;
 struct bpe_handle {
     int device = 0;
-    EncState *enc = nullptr;          // memoised chunk encode (encode2_host.inl): rank table, memo, id pool, scratch
-    bpe_handle *enc_scratch = nullptr;   // general encode path (encode_host.inl) works on its own stream buffers
-    SpecSet *spec = nullptr;             // special tokens of the current encode call (special_host.inl)
-    GenEnc *gen = nullptr;               // general encode path: device scratch + the rank table of the last merges seen (encode_host.inl)
-    DdSession *dd = nullptr;             // counting session of bpe_dedup_begin / _add_docs / _finish (dedup_host.inl)
+    std::unique_ptr<EncState> enc;       // memoised chunk encode (encode2_host.inl): rank table, memo, id pool, scratch
+    std::unique_ptr<bpe_handle, int (*)(bpe_handle *)> enc_scratch{nullptr, bpe_destroy};   // general encode path
+                                         // (encode_host.inl) works on its own stream buffers
+    std::unique_ptr<SpecSet> spec;       // special tokens of the current encode call (special_host.inl)
+    std::unique_ptr<GenEnc> gen;         // general encode path: device scratch + the rank table of the last merges seen (encode_host.inl)
+    std::unique_ptr<DdSession> dd;       // counting session of bpe_dedup_begin / _add_docs / _finish (dedup_host.inl)
     int sms = 0;
     cudaStream_t stream = nullptr;       // the stream every kernel of this handle runs on
     cudaStream_t own_stream = nullptr;   // created by bpe_create; `stream` may point at a caller's stream instead
     std::string err;
 
-    // token stream: two ping-pong buffers of cap_tokens words
-    u32 *buf[2] = {nullptr, nullptr};
-    u64 cap_tokens = 0;
+    // token stream: two ping-pong buffers
+    DevBuf<u32> buf[2];
     bool loaded = false;
     bool bytes_only = false;  // every id < 256 (fresh byte stream)
     // weighted stream (bpe_load_chunks_weighted, k_weighted.cuh): one weight per entry, the entry base of every segment
     bool weighted = false;
-    u64 *wts = nullptr; u64 wts_cap = 0, n_entries = 0;
-    u32 *wt_cnt = nullptr; u64 *wt_base = nullptr; u64 wt_seg_cap = 0;
+    DevBuf<u64> wts; u64 n_entries = 0;
+    DevBuf<u32> wt_cnt; DevBuf<u64> wt_base;
     bool wt_fresh = false;    // the weighted stream is as loaded: no bpe_train / bpe_replay since (bpe_read_chunk_entries)
 
-    Ctl *ctl = nullptr;    // device
+    DevBuf<Ctl> ctl;       // device
     Ctl *h_ctl = nullptr;  // pinned host mirror
 
-    Table table = {nullptr, nullptr, nullptr, 0};
+    PairTable table;
     bool table_valid = false;  // table == get_stats(current stream)
-    u64 *desc = nullptr; u64 desc_cap = 0;
-    Edge *edge[2] = {nullptr, nullptr}; u64 *seg_offs = nullptr; u64 seg_cap = 0;  // segmented stream metadata
-    ull *delta = nullptr; u32 V = 0;   // V = layout of the delta vector the kernels index (L[0,V) R[V,2V) ZZ[2V])
+    DevBuf<u64> desc;
+    DevBuf<Edge> edge[2]; DevBuf<u64> seg_offs;   // segmented stream metadata
+    DevBuf<ull> delta; u32 V = 0;      // V = layout of the delta vector the kernels index (L[0,V) R[V,2V) ZZ[2V])
     u32 delta_cap = 0;                 // vocabulary capacity of the OWNED buffer `delta` (step mode uses the caller's)
     u32 delta_vecs = 0;                // delta vectors of 2*delta_cap+1 counters in it: one per member of a batched pass
     bool batching = false;             // bpe_train's loop may carry several merges per pass (k_select_batch)
     u32 max_id = 255;                  // largest id in the loaded stream (bpe_load_ids); byte streams: 255
-    ull *dense = nullptr;
-    ull *dense2 = nullptr; u32 *d_cmp = nullptr;   // first-use cross-check of the packed histogram kernel (hist_dense)
+    DevBuf<ull> dense;
+    DevBuf<ull> dense2; DevBuf<u32> d_cmp;         // first-use cross-check of the packed histogram kernel (hist_dense)
     int hist_mode = 0;                             // 0 = not decided, 1 = k_hist_dense_packed, 2 = k_hist_dense
     // segment filter (k_seg_filter.cuh): signatures, candidate list
-    u32 *sig = nullptr, *cand = nullptr; u64 sig_cap = 0;
+    DevBuf<u32> sig, cand;
     bool filt_active = false;                      // the iterations being enqueued use the filter
     bool sig_valid = false;                        // the signatures describe the current stream
-    u32 *d_err = nullptr;
-    int *log_pairs = nullptr; long long *log_counts = nullptr; int log_cap = 0;
-    Best *partials = nullptr;
-    TopList *top_partials = nullptr;   // k_select_batch: one list per block
-    unsigned char *d_cls = nullptr, *d_contr = nullptr;   // code-point class / contraction tables of the GPT-4 splitter
+    DevBuf<u32> d_err;
+    DevBuf<int> log_pairs; DevBuf<long long> log_counts;
+    DevBuf<Best> partials;
+    DevBuf<TopList> top_partials;      // k_select_batch: one list per block
+    DevBuf<unsigned char> d_cls, d_contr;   // code-point class / contraction tables of the GPT-4 splitter
     // sharded loop over NVLink peer memory (k_xchg.cuh): the rank's exchange block and its peers' mappings
     unsigned char *xchg = nullptr; u64 xchg_bytes = 0, xchg_stride = 0; u32 xchg_V = 0;
     XArgs xargs = {};
     bool xchg_attached = false;
-    u32 *d_present = nullptr;   // sharded loop: bitmap of pair hashes that have occurred in this shard (k_stats.cuh)
-    unsigned char *split_slab = nullptr; u64 split_cap = 0;   // working set of the splitter, kept between calls (split_host.inl)
+    DevBuf<u32> d_present;      // sharded loop: bitmap of pair hashes that have occurred in this shard (k_stats.cuh)
+    DevBuf<unsigned char> split_slab;   // working set of the splitter, kept between calls (split_host.inl)
     int argmax_grid = 0, merge_grid_same = 0, merge_grid_seg = 0, ff_grid = 0;
 
     // options
@@ -101,16 +145,14 @@ struct bpe_handle {
     int opt_split_pattern = 0;   // BPE_OPT_SPLIT_PATTERN: 0 = GPT-4 split pattern, 1 = GPT-2 (bpe_split_gpt4 / bpe_load_text_gpt4 / bpe_encode_text_gpt4*)
 
     bpe_timing tm = {};
-    std::vector<cudaEvent_t> ev_pool;  // per-launch timing of the fused merge kernel (BPE_OPT_KERNEL_TIMING)
+    std::vector<Event> ev_pool;  // per-launch timing of the fused merge kernel (BPE_OPT_KERNEL_TIMING)
     int ev_used = 0;
+
+    __attribute__((visibility("hidden"))) ~bpe_handle();   // after the .inl files, where the sub-states are complete types
 };
 
 static thread_local std::string g_create_err;
 static void xchg_release(bpe_handle *h);
-static void enc2_free(bpe_handle *h);
-static void spec_free(bpe_handle *h);
-static void gen_free(bpe_handle *h);
-static void dd_free(bpe_handle *h);
 static u64 g_split_piece_override = 0;   // BPE_OPT_SPLIT_PIECE (test hook): bytes per piece of the device splitter
 
 static int fail(bpe_handle *h, int code, const std::string &msg) {
@@ -137,20 +179,44 @@ extern "C" int bpe_abi_version(void) { return BPE_ABI_VERSION; }
 extern "C" const char *bpe_last_error(const bpe_handle *h) { return h ? h->err.c_str() : g_create_err.c_str(); }
 
 // ------------------------------------------------------------------------------------------------
-static int free_table(bpe_handle *h, Table &t) {
-    if (t.keys) cudaFree(t.keys);
-    if (t.counts) cudaFree(t.counts);
-    if (t.first) cudaFree(t.first);
-    t = {nullptr, nullptr, nullptr, 0};
-    (void)h;
+// Room for `need` elements; the contents are not kept.  A buffer that is too small is freed FIRST and then allocated
+// again with `alloc` elements (default: `need`), so the old and the new block never coexist; if that fails, the buffer is
+// left empty.
+template <class T>
+static int dev_reserve(bpe_handle *h, DevBuf<T> &b, u64 need, u64 alloc = 0) {
+    if (need <= b.cap) return BPE_OK;
+    b.reset();
+    const u64 n = std::max(need, alloc);
+    T *q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, n * sizeof(T));
+    if (e != cudaSuccess)
+        return fail(h, BPE_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    b.p = q; b.cap = n;
     return BPE_OK;
 }
 
-static int alloc_table(bpe_handle *h, Table &t, u64 cap, bool with_first) {
-    t = {nullptr, nullptr, nullptr, cap - 1};
-    CU(cudaMalloc(&t.keys, cap * 8));
-    CU(cudaMalloc(&t.counts, cap * 8));
-    if (with_first) CU(cudaMalloc(&t.first, cap * 8));
+// Room for `need` elements, keeping the first `used`: the buffer at least doubles when it grows.
+template <class T>
+static int dev_grow(bpe_handle *h, DevBuf<T> &b, u64 need, u64 used) {
+    if (need <= b.cap) return BPE_OK;
+    DevBuf<T> nb;
+    int rc = dev_reserve(h, nb, std::max<u64>(need, 1), b.cap * 2);
+    if (rc) return rc;
+    if (used) CU(cudaMemcpyAsync(nb, b, used * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    b = std::move(nb);
+    return BPE_OK;
+}
+
+// `cap` empty slots (with_first: first positions too); arrays of another size are freed before the new ones are allocated
+static int table_reset(bpe_handle *h, PairTable &t, u64 cap, bool with_first) {
+    if (!t.keys || t.mask + 1 != cap) {
+        t = PairTable();
+        int rc;
+        if ((rc = dev_reserve(h, t.keys, cap)) || (rc = dev_reserve(h, t.counts, cap)) ||
+            (with_first && (rc = dev_reserve(h, t.first, cap)))) { t = PairTable(); return rc; }
+        t.mask = cap - 1;
+    }
     CU(cudaMemsetAsync(t.keys, 0xff, cap * 8, h->stream));
     CU(cudaMemsetAsync(t.counts, 0, cap * 8, h->stream));
     if (with_first) CU(cudaMemsetAsync(t.first, 0xff, cap * 8, h->stream));
@@ -159,27 +225,39 @@ static int alloc_table(bpe_handle *h, Table &t, u64 cap, bool with_first) {
 
 static u64 next_pow2(u64 x) { u64 p = 1; while (p < x) p <<= 1; return p; }
 
-// grow-only device buffer of `elem`-byte elements; the first `used` elements are kept
-struct DevBuf {
-    void *p = nullptr; u64 cap = 0;
-    ~DevBuf() { if (p) cudaFree(p); }
-    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
-};
-static int dev_grow(bpe_handle *h, DevBuf &b, u64 need, u64 used, size_t elem) {
-    if (need <= b.cap) return BPE_OK;
-    const u64 nc = std::max<u64>(need, b.cap * 2);
-    void *q = nullptr;
-    CU(cudaMalloc(&q, std::max<u64>(nc, 1) * elem));
-    cudaError_t e = used ? cudaMemcpyAsync(q, b.p, used * elem, cudaMemcpyDeviceToDevice, h->stream) : cudaSuccess;
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e != cudaSuccess) { cudaFree(q); return fail(h, BPE_ERR_CUDA, std::string("dev_grow: ") + cudaGetErrorString(e)); }
-    if (b.p) cudaFree(b.p);
-    b.p = q; b.cap = nc;
+// stream, control block, histogram scratch, launch geometry of a new handle; errors go to h->err
+static int handle_init(bpe_handle *h, int device, const cudaDeviceProp &prop) {
+    h->device = device;
+    h->sms = prop.multiProcessorCount;
+    CU(cudaSetDevice(device));
+    CU(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
+    h->stream = h->own_stream;
+    int rc;
+    if ((rc = dev_reserve(h, h->ctl, 1))) return rc;
+    CU(cudaMallocHost(&h->h_ctl, sizeof(Ctl)));
+    if ((rc = dev_reserve(h, h->dense, 65536)) || (rc = dev_reserve(h, h->d_err, 2)))   // d_err: [0] error flag, [1] max id seen by k_copy_ids
+        return rc;
+    int occ_same = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_same, k_merge<true>, MG_THREADS, 0);
+    if (occ_same < 1) occ_same = 1;
+    h->merge_grid_same = h->sms * occ_same;
+    int occ_fast = 0;
+    CU(cudaFuncSetAttribute(k_merge_seg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES));
+    CU(cudaFuncSetAttribute(k_merge_seg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES));
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_fast, k_merge_seg<false>, MS_THREADS, MS_SMEM_BYTES);
+    if (occ_fast < 1) return fail(h, BPE_ERR_CUDA, "k_merge_seg does not fit on an SM");
+    h->merge_grid_seg = h->sms * occ_fast;
+    h->argmax_grid = h->sms * 2;
+    h->ff_grid = h->sms * 4;
+    if ((rc = dev_reserve(h, h->partials, h->argmax_grid)) || (rc = dev_reserve(h, h->top_partials, h->argmax_grid))) return rc;
+    memset(h->h_ctl, 0, sizeof(Ctl));
+    h->h_ctl->epoch = 1;
+    h->h_ctl->found_pos = POS_NONE;
+    CU(cudaMemcpy(h->ctl, h->h_ctl, sizeof(Ctl), cudaMemcpyHostToDevice));
     return BPE_OK;
 }
 
 extern "C" int bpe_create(int device, bpe_handle **out) {
-    bpe_handle *h = nullptr;
     if (!out) return fail(nullptr, BPE_ERR_ARG, "bpe_create: out is NULL");
     *out = nullptr;
     int ndev = 0;
@@ -195,42 +273,10 @@ extern "C" int bpe_create(int device, bpe_handle **out) {
         return fail(nullptr, BPE_ERR_CUDA, std::string("bpe_create: device '") + prop.name + "' is sm_" +
                                                std::to_string(prop.major) + std::to_string(prop.minor) +
                                                "; this library contains sm_90a code only");
-    h = new (std::nothrow) bpe_handle();
-    if (!h) return fail(nullptr, BPE_ERR_INTERNAL, "out of host memory");
-    h->device = device;
-    h->sms = prop.multiProcessorCount;
-    auto bail = [&](const char *what, cudaError_t ce) {
-        std::string m = std::string(what) + ": " + cudaGetErrorString(ce);
-        delete h;
-        return fail(nullptr, BPE_ERR_CUDA, m);
-    };
-    if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
-    if ((e = cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
-    h->stream = h->own_stream;
-    if ((e = cudaMalloc(&h->ctl, sizeof(Ctl))) != cudaSuccess) return bail("cudaMalloc ctl", e);
-    if ((e = cudaMallocHost(&h->h_ctl, sizeof(Ctl))) != cudaSuccess) return bail("cudaMallocHost", e);
-    if ((e = cudaMalloc(&h->dense, 65536 * 8)) != cudaSuccess) return bail("cudaMalloc dense", e);
-    if ((e = cudaMalloc(&h->d_err, 8)) != cudaSuccess) return bail("cudaMalloc err", e);   // [0] error flag, [1] max id seen by k_copy_ids
-    int occ_same = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_same, k_merge<true>, MG_THREADS, 0);
-    if (occ_same < 1) occ_same = 1;
-    h->merge_grid_same = h->sms * occ_same;
-    int occ_fast = 0;
-    if ((e = cudaFuncSetAttribute(k_merge_seg<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES)) != cudaSuccess ||
-        (e = cudaFuncSetAttribute(k_merge_seg<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MS_SMEM_BYTES)) != cudaSuccess)
-        return bail("cudaFuncSetAttribute(k_merge_seg)", e);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_fast, k_merge_seg<false>, MS_THREADS, MS_SMEM_BYTES);
-    if (occ_fast < 1) return bail("k_merge_seg does not fit on an SM", cudaErrorLaunchOutOfResources);
-    h->merge_grid_seg = h->sms * occ_fast;
-    h->argmax_grid = h->sms * 2;
-    h->ff_grid = h->sms * 4;
-    if ((e = cudaMalloc(&h->partials, sizeof(Best) * h->argmax_grid)) != cudaSuccess) return bail("cudaMalloc partials", e);
-    if ((e = cudaMalloc(&h->top_partials, sizeof(TopList) * h->argmax_grid)) != cudaSuccess) return bail("cudaMalloc top_partials", e);
-    memset(h->h_ctl, 0, sizeof(Ctl));
-    h->h_ctl->epoch = 1;
-    h->h_ctl->found_pos = POS_NONE;
-    if ((e = cudaMemcpy(h->ctl, h->h_ctl, sizeof(Ctl), cudaMemcpyHostToDevice)) != cudaSuccess) return bail("cudaMemcpy ctl", e);
-    *out = h;
+    std::unique_ptr<bpe_handle> owner(new (std::nothrow) bpe_handle());   // frees whatever was made if a step fails
+    if (!owner) return fail(nullptr, BPE_ERR_INTERNAL, "out of host memory");
+    if (int rc = handle_init(owner.get(), device, prop)) return fail(nullptr, rc, owner->err);
+    *out = owner.release();
     return BPE_OK;
 }
 
@@ -238,40 +284,8 @@ extern "C" int bpe_destroy(bpe_handle *h) {
     if (!h) return BPE_OK;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
-    for (int i = 0; i < 2; ++i) if (h->buf[i]) cudaFree(h->buf[i]);
-    for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
-    free_table(h, h->table);
-    if (h->desc) cudaFree(h->desc);
-    for (int i = 0; i < 2; ++i) if (h->edge[i]) cudaFree(h->edge[i]);
-    if (h->seg_offs) cudaFree(h->seg_offs);
-    if (h->sig) cudaFree(h->sig);
-    if (h->cand) cudaFree(h->cand);
-    if (h->delta) cudaFree(h->delta);
-    if (h->dense) cudaFree(h->dense);
-    if (h->dense2) cudaFree(h->dense2);
-    if (h->d_cmp) cudaFree(h->d_cmp);
-    if (h->d_err) cudaFree(h->d_err);
-    if (h->log_pairs) cudaFree(h->log_pairs);
-    if (h->log_counts) cudaFree(h->log_counts);
-    if (h->partials) cudaFree(h->partials);
-    if (h->top_partials) cudaFree(h->top_partials);
-    if (h->d_cls) cudaFree(h->d_cls);
-    if (h->d_contr) cudaFree(h->d_contr);
-    if (h->d_present) cudaFree(h->d_present);
-    if (h->wts) cudaFree(h->wts);
-    if (h->wt_cnt) cudaFree(h->wt_cnt);
-    if (h->wt_base) cudaFree(h->wt_base);
     xchg_release(h);
-    enc2_free(h);
-    spec_free(h);
-    gen_free(h);
-    dd_free(h);
-    if (h->enc_scratch) bpe_destroy(h->enc_scratch);
-    if (h->split_slab) cudaFree(h->split_slab);
-    if (h->ctl) cudaFree(h->ctl);
-    if (h->h_ctl) cudaFreeHost(h->h_ctl);
-    if (h->own_stream) cudaStreamDestroy(h->own_stream);
-    delete h;
+    delete h;   // every buffer, event and sub-state has its owner in the handle
     return BPE_OK;
 }
 
@@ -291,7 +305,7 @@ extern "C" int bpe_set_option(bpe_handle *h, int opt, int64_t value) {
             if (value != 0 && (value < 6 || value > 28)) return fail(h, BPE_ERR_ARG, "memo log2 must be 0 or in [6,28]");
             h->opt_memo_log2 = (int)value;
             cudaSetDevice(h->device); cudaStreamSynchronize(h->stream);
-            enc2_free(h);   // re-created with the new size by the next encode call
+            h->enc.reset();   // re-created with the new size by the next encode call
             break;
         case BPE_OPT_SEG_FILTER:
             if (value < 0 || value > 2) return fail(h, BPE_ERR_ARG, "segment filter must be 0 (off), 1 (when sparse) or 2 (always)");
@@ -327,29 +341,22 @@ extern "C" int bpe_get_timing(bpe_handle *h, bpe_timing *out) {
 static int ensure_stream_capacity(bpe_handle *h, u64 n) {
     // round up to whole tiles (+ slack) so 16-byte loads at the tail stay inside the allocation
     const u64 need = ((n + MG_TILE - 1) / MG_TILE + 1) * MG_TILE;
-    if (need > h->cap_tokens) {
-        if (h->split_slab) { cudaFree(h->split_slab); h->split_slab = nullptr; h->split_cap = 0; }   // make room first
-        for (int i = 0; i < 2; ++i) { if (h->buf[i]) cudaFree(h->buf[i]); h->buf[i] = nullptr; }
-        h->cap_tokens = 0;
-        for (int i = 0; i < 2; ++i) CU(cudaMalloc(&h->buf[i], need * 4));
-        h->cap_tokens = need;
+    int rc;
+    if (need > h->buf[0].cap || need > h->buf[1].cap) {
+        // make room first: the splitter's slab and both old buffers go before the new ones are allocated
+        h->split_slab.reset(); h->buf[0].reset(); h->buf[1].reset();
+        if ((rc = dev_reserve(h, h->buf[0], need)) || (rc = dev_reserve(h, h->buf[1], need))) return rc;
     }
     const u64 tiles = need / MG_TILE + 1;
-    if (tiles > h->desc_cap) {
-        if (h->desc) cudaFree(h->desc);
-        h->desc = nullptr; h->desc_cap = 0;
-        CU(cudaMalloc(&h->desc, tiles * 8));
+    if (tiles > h->desc.cap) {
+        if ((rc = dev_reserve(h, h->desc, tiles))) return rc;
         CU(cudaMemsetAsync(h->desc, 0, tiles * 8, h->stream));
-        h->desc_cap = tiles;
     }
     const u64 segs = need / SEG_TOKENS + 1;
-    if (segs > h->seg_cap) {
-        for (int i = 0; i < 2; ++i) { if (h->edge[i]) cudaFree(h->edge[i]); h->edge[i] = nullptr; }
-        if (h->seg_offs) cudaFree(h->seg_offs);
-        h->seg_offs = nullptr; h->seg_cap = 0;
-        for (int i = 0; i < 2; ++i) CU(cudaMalloc(&h->edge[i], segs * sizeof(Edge)));
-        CU(cudaMalloc(&h->seg_offs, segs * 8));
-        h->seg_cap = segs;
+    if (segs > h->edge[0].cap || segs > h->edge[1].cap || segs > h->seg_offs.cap) {
+        h->edge[0].reset(); h->edge[1].reset(); h->seg_offs.reset();
+        if ((rc = dev_reserve(h, h->edge[0], segs)) || (rc = dev_reserve(h, h->edge[1], segs)) || (rc = dev_reserve(h, h->seg_offs, segs)))
+            return rc;
     }
     return BPE_OK;
 }
@@ -416,38 +423,32 @@ static int mark_chunks(bpe_handle *h, u32 *dst, const uint64_t *offs, uint64_t k
     if (!offs || k == 0) { offs = &zero; k = n ? 1 : 0; }
     if (k == 0) return BPE_OK;
     const u64 piece = 1ull << 24;  // 16M offsets = 128 MB per piece
-    u64 *d_offs = nullptr;
-    CU(cudaMalloc(&d_offs, std::min(piece, k) * 8));
+    DevBuf<u64> d_offs;
+    int rc = dev_reserve(h, d_offs, std::min(piece, k));
+    if (rc) return rc;
     for (u64 s = 0; s < k; s += piece) {
         const u64 m = std::min(piece, k - s);
-        cudaError_t e = cudaMemcpyAsync(d_offs, offs + s, m * 8, cudaMemcpyHostToDevice, h->stream);
-        if (e == cudaSuccess) {
-            k_set_flags<<<grid_for(m, 256, h->sms * 8), 256, 0, h->stream>>>(dst, d_offs, m, n);
-            e = cudaStreamSynchronize(h->stream);
-        }
-        if (e != cudaSuccess) { cudaFree(d_offs); return fail(h, BPE_ERR_CUDA, std::string("mark_chunks: ") + cudaGetErrorString(e)); }
+        CU(cudaMemcpyAsync(d_offs, offs + s, m * 8, cudaMemcpyHostToDevice, h->stream));
+        k_set_flags<<<grid_for(m, 256, h->sms * 8), 256, 0, h->stream>>>(dst, d_offs, m, n);
+        CU(cudaStreamSynchronize(h->stream));
         h->tm.h2d_bytes += m * 8;
     }
-    cudaFree(d_offs);
     return BPE_OK;
 }
 
 static int load_bytes_into(bpe_handle *h, u32 *dst, const uint8_t *bytes, uint64_t n, const unsigned char *d_perm) {
     const u64 piece = 1ull << 28;  // 256 MiB of text per staging copy
-    unsigned char *d_bytes = nullptr;
     if (n == 0) return BPE_OK;
-    CU(cudaMalloc(&d_bytes, std::min(piece, n)));
+    DevBuf<unsigned char> d_bytes;
+    int rc = dev_reserve(h, d_bytes, std::min(piece, n));
+    if (rc) return rc;
     for (u64 s = 0; s < n; s += piece) {
         const u64 m = std::min(piece, n - s);
-        cudaError_t e = cudaMemcpyAsync(d_bytes, bytes + s, m, cudaMemcpyHostToDevice, h->stream);
-        if (e == cudaSuccess) {
-            k_widen_bytes<<<grid_for(m / 16 + 1, 256, h->sms * 8), 256, 0, h->stream>>>(d_bytes, dst + s, m, d_perm);
-            e = cudaStreamSynchronize(h->stream);
-        }
-        if (e != cudaSuccess) { cudaFree(d_bytes); return fail(h, BPE_ERR_CUDA, std::string("load_bytes: ") + cudaGetErrorString(e)); }
+        CU(cudaMemcpyAsync(d_bytes, bytes + s, m, cudaMemcpyHostToDevice, h->stream));
+        k_widen_bytes<<<grid_for(m / 16 + 1, 256, h->sms * 8), 256, 0, h->stream>>>(d_bytes, dst + s, m, d_perm);
+        CU(cudaStreamSynchronize(h->stream));
         h->tm.h2d_bytes += m;
     }
-    cudaFree(d_bytes);
     return BPE_OK;
 }
 
@@ -486,7 +487,7 @@ extern "C" int bpe_load_ids(bpe_handle *h, const int32_t *ids, uint64_t n, const
         // stage through buf[1] (same size), then convert into buf[0]
         CU(cudaMemcpyAsync(h->buf[1], ids, n * 4, cudaMemcpyHostToDevice, h->stream));
         CU(cudaMemsetAsync(h->d_err, 0, 8, h->stream));
-        k_copy_ids<<<grid_for(n, 256, h->sms * 8), 256, 0, h->stream>>>((const int *)h->buf[1], h->buf[0], n, h->d_err);
+        k_copy_ids<<<grid_for(n, 256, h->sms * 8), 256, 0, h->stream>>>((const int *)h->buf[1].p, h->buf[0], n, h->d_err);
         u32 bad[2] = {0, 0};
         CU(cudaMemcpyAsync(bad, h->d_err, 8, cudaMemcpyDeviceToHost, h->stream));
         CU(cudaStreamSynchronize(h->stream));
@@ -528,7 +529,7 @@ extern "C" int bpe_read_stream(bpe_handle *h, int32_t *out, uint64_t cap, uint64
     k_scan_counts<<<1, 1024, 0, h->stream>>>(h->ctl, h->edge[0], h->edge[1], h->seg_offs, 1);
     k_gather<<<h->sms * 8, 256, 0, h->stream>>>(h->ctl, h->buf[0], h->buf[1], h->edge[0], h->edge[1], h->seg_offs,
                                                  h->buf[cur ^ 1], 1, 0);
-    k_strip_flags<<<grid_for(len, 256, h->sms * 8), 256, 0, h->stream>>>(h->buf[cur ^ 1], (int *)h->buf[cur ^ 1], len);
+    k_strip_flags<<<grid_for(len, 256, h->sms * 8), 256, 0, h->stream>>>(h->buf[cur ^ 1], (int *)h->buf[cur ^ 1].p, len);
     CU(cudaMemcpyAsync(out, h->buf[cur ^ 1], len * 4, cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     h->tm.d2h_bytes = len * 4;
@@ -537,23 +538,11 @@ extern "C" int bpe_read_stream(bpe_handle *h, int32_t *out, uint64_t cap, uint64
 
 // ------------------------------------------------------------------------------------------------
 // weighted stream (k_weighted.cuh): entries = chunk occurrences in text order, each standing for `weight` occurrences
-// storage of a weighted stream of n_entries entries over the stream just loaded (its segments: h->seg_cap)
+// storage of a weighted stream of n_entries entries over the stream just loaded (its segments: h->seg_offs.cap)
 static int wt_alloc(bpe_handle *h, u64 n_entries) {
-    if (n_entries > h->wts_cap) {
-        if (h->wts) cudaFree(h->wts);
-        h->wts = nullptr; h->wts_cap = 0;
-        CU(cudaMalloc(&h->wts, n_entries * 8));
-        h->wts_cap = n_entries;
-    }
-    if (h->seg_cap > h->wt_seg_cap) {
-        if (h->wt_cnt) cudaFree(h->wt_cnt);
-        if (h->wt_base) cudaFree(h->wt_base);
-        h->wt_cnt = nullptr; h->wt_base = nullptr; h->wt_seg_cap = 0;
-        CU(cudaMalloc(&h->wt_cnt, h->seg_cap * 4));
-        CU(cudaMalloc(&h->wt_base, h->seg_cap * 8));
-        h->wt_seg_cap = h->seg_cap;
-    }
-    return BPE_OK;
+    int rc = dev_reserve(h, h->wts, n_entries);
+    if (!rc) rc = dev_reserve(h, h->wt_cnt, h->seg_offs.cap);
+    return rc ? rc : dev_reserve(h, h->wt_base, h->seg_offs.cap);
 }
 // the weights are in h->wts: entry bases, and the handle holds a weighted stream
 static int wt_finish(bpe_handle *h, u64 n_entries) {
@@ -628,8 +617,8 @@ extern "C" int bpe_get_stats(bpe_handle *h, int32_t *pairs, int64_t *counts, uin
     const u64 n = h->h_ctl->n;
     // distinct pairs <= n - 1; keep the load factor <= 0.5
     const u64 tcap = next_pow2(std::max<u64>(1024, 2 * n));
-    Table t;
-    if ((rc = alloc_table(h, t, tcap, true))) { free_table(h, t); return rc; }
+    PairTable t;
+    if ((rc = table_reset(h, t, tcap, true))) return rc;
     const u64 used_before = h->h_ctl->table_used;
     {   // the scratch table counts its own occupancy (k_hist_hash refuses inserts near a full table)
         const ull zero = 0;
@@ -637,15 +626,13 @@ extern "C" int bpe_get_stats(bpe_handle *h, int32_t *pairs, int64_t *counts, uin
     }
     k_hist_hash<<<h->sms * 8, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], t, 0);
     std::vector<u64> keys(tcap), cnt(tcap), first(tcap);
-    cudaError_t e = cudaMemcpyAsync(keys.data(), t.keys, tcap * 8, cudaMemcpyDeviceToHost, h->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(cnt.data(), t.counts, tcap * 8, cudaMemcpyDeviceToHost, h->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(first.data(), t.first, tcap * 8, cudaMemcpyDeviceToHost, h->stream);
+    CU(cudaMemcpyAsync(keys.data(), t.keys, tcap * 8, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaMemcpyAsync(cnt.data(), t.counts, tcap * 8, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaMemcpyAsync(first.data(), t.first, tcap * 8, cudaMemcpyDeviceToHost, h->stream));
     // k_hist_hash bumped ctl->table_used for the scratch table: restore it
     h->h_ctl->table_used = used_before;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h->ctl->table_used, &h->h_ctl->table_used, 8, cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    free_table(h, t);
-    if (e != cudaSuccess) return fail(h, BPE_ERR_CUDA, std::string("bpe_get_stats: ") + cudaGetErrorString(e));
+    CU(cudaMemcpyAsync(&h->ctl->table_used, &h->h_ctl->table_used, 8, cudaMemcpyHostToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
     std::vector<u64> order;
     for (u64 i = 0; i < tcap; ++i) if (keys[i] != KEY_EMPTY) order.push_back(i);
     std::sort(order.begin(), order.end(), [&](u64 x, u64 y) { return first[x] < first[y]; });
@@ -751,9 +738,9 @@ static u64 auto_table_cap(bpe_handle *h, u64 n_unbounded_inserts) {
 static int ensure_delta(bpe_handle *h, u32 V, u32 vecs = 1) {
     bool fresh = false;
     if (!h->delta || h->delta_cap < V || h->delta_vecs < vecs) {
-        if (h->delta) cudaFree(h->delta);
-        h->delta = nullptr; h->delta_cap = 0; h->delta_vecs = 0;
-        CU(cudaMalloc(&h->delta, (u64)vecs * (2ull * V + 1) * 8));
+        h->delta.reset(); h->delta_cap = 0; h->delta_vecs = 0;   // sized for (V, vecs) exactly, also when that is smaller
+        int rc = dev_reserve(h, h->delta, (u64)vecs * (2ull * V + 1));
+        if (rc) return rc;
         h->delta_cap = V; h->delta_vecs = vecs;
         fresh = true;
     }
@@ -761,6 +748,11 @@ static int ensure_delta(bpe_handle *h, u32 V, u32 vecs = 1) {
         CU(cudaMemsetAsync(h->delta, 0, (u64)h->delta_vecs * (2ull * h->delta_cap + 1) * 8, h->stream));
     h->V = V;
     return BPE_OK;
+}
+// the device log of the merges of one run (bpe_train, the step API): a pair and its count per merge
+static int ensure_log(bpe_handle *h, int num_merges) {
+    const int rc = dev_reserve(h, h->log_pairs, 2ull * num_merges);
+    return rc ? rc : dev_reserve(h, h->log_counts, (u64)num_merges);
 }
 // Batched passes index BATCH_MAX delta vectors with one 32-bit flat index (the merge kernel's shared-memory cache keys,
 // 0xffffffff = empty) and allocate them all: vocabularies up to 2^21 ids.
@@ -785,21 +777,19 @@ static int hist_dense(bpe_handle *h, ull *dense_out) {
     if (h->hist_mode == 0 && h->h_ctl->n >= HIST_DECIDE_MIN_TOKENS) {
         h->hist_mode = 2;
         if (cudaFuncSetAttribute(k_hist_dense_packed, cudaFuncAttributeMaxDynamicSharedMemorySize, HP_SMEM_BYTES) == cudaSuccess) {
-            if (!h->dense2) CU(cudaMalloc(&h->dense2, 65536 * 8));
-            if (!h->d_cmp) CU(cudaMalloc(&h->d_cmp, 4));
+            int rc;
+            if ((rc = dev_reserve(h, h->dense2, 65536)) || (rc = dev_reserve(h, h->d_cmp, 1))) return rc;
             CU(cudaMemsetAsync(h->dense2, 0, 65536 * 8, h->stream));
             CU(cudaMemsetAsync(h->d_cmp, 0, 4, h->stream));
-            cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-            for (auto &e : ev) CU(cudaEventCreate(&e));
-            auto drop_events = [&]() { for (auto &e : ev) cudaEventDestroy(e); };
+            Event ev[3];
+            for (auto &e : ev) CU(e.create());
             cudaEventRecord(ev[0], h->stream);
             k_hist_dense<<<grid_old, 256, 0, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], dense_out, h->d_err);
             cudaEventRecord(ev[1], h->stream);
-            if (cudaGetLastError() != cudaSuccess) { drop_events(); return fail(h, BPE_ERR_CUDA, "k_hist_dense launch failed"); }
+            if (cudaGetLastError() != cudaSuccess) return fail(h, BPE_ERR_CUDA, "k_hist_dense launch failed");
             k_hist_dense_packed<<<h->sms, HP_THREADS, HP_SMEM_BYTES, h->stream>>>(h->buf[0], h->buf[1], h->ctl, h->edge[0], h->edge[1], h->dense2, h->d_err);
             cudaEventRecord(ev[2], h->stream);
             if (cudaGetLastError() != cudaSuccess) {      // the launch itself was refused (a launch error is not sticky): keep k_hist_dense
-                drop_events();
                 h->tm.kernel_launches += 1;
                 h->tm.hist_kernel = 2;
                 return BPE_OK;
@@ -811,7 +801,6 @@ static int hist_dense(bpe_handle *h, ull *dense_out) {
             if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
             float ms_old = 0, ms_new = 0;
             if (e == cudaSuccess) { cudaEventElapsedTime(&ms_old, ev[0], ev[1]); cudaEventElapsedTime(&ms_new, ev[1], ev[2]); }
-            drop_events();
             if (e != cudaSuccess) return fail(h, BPE_ERR_CUDA, std::string("hist_dense: ") + cudaGetErrorString(e));
             // adopted only when it gives the same 65,536 counters AND is not slower on this very stream
             if (!differ && ms_new <= ms_old) h->hist_mode = 1;
@@ -831,13 +820,7 @@ static int hist_dense(bpe_handle *h, ull *dense_out) {
 // (re)build the pair-count table from the current stream
 static int build_table(bpe_handle *h, u64 cap) {
     int rc;
-    if (!h->table.keys || h->table.mask + 1 != cap) {
-        free_table(h, h->table);
-        if ((rc = alloc_table(h, h->table, cap, false))) return rc;
-    } else {
-        CU(cudaMemsetAsync(h->table.keys, 0xff, cap * 8, h->stream));
-        CU(cudaMemsetAsync(h->table.counts, 0, cap * 8, h->stream));
-    }
+    if ((rc = table_reset(h, h->table, cap, false))) return rc;
     const ull zero = 0;
     CU(cudaMemcpyAsync(&h->ctl->table_used, &zero, 8, cudaMemcpyHostToDevice, h->stream));
     if (h->weighted) {      // weighted sums straight into the table; takes no part in the choice of hist_dense
@@ -860,16 +843,15 @@ static int build_table(bpe_handle *h, u64 cap) {
 
 // grow / clean the table: live entries are re-inserted into a fresh table of `cap` slots
 static int rehash_table(bpe_handle *h, u64 cap) {
-    Table nt;
-    int rc = alloc_table(h, nt, cap, false);
-    if (rc) { free_table(h, nt); return rc; }
+    PairTable nt;
+    int rc = table_reset(h, nt, cap, false);
+    if (rc) return rc;
     const ull zero = 0;
     CU(cudaMemcpyAsync(&h->ctl->table_used, &zero, 8, cudaMemcpyHostToDevice, h->stream));
     k_rehash<<<grid_for(h->table.mask + 1, 256, h->sms * 8), 256, 0, h->stream>>>(h->table, nt, h->ctl);
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(h->stream));
-    free_table(h, h->table);
-    h->table = nt;
+    h->table = std::move(nt);
     h->tm.kernel_launches++;
     return BPE_OK;
 }
@@ -885,7 +867,7 @@ static void drain_kernel_events(bpe_handle *h) {
 
 static void timed_merge(bpe_handle *h, ull *delta, bool use_xchg = false, bool batched = false) {
     if (!h->opt_kernel_timing) { launch_merge(h, delta, 0, -1, use_xchg, batched); return; }
-    while ((int)h->ev_pool.size() < h->ev_used + 2) { cudaEvent_t e; cudaEventCreate(&e); h->ev_pool.push_back(e); }
+    while ((int)h->ev_pool.size() < h->ev_used + 2) { h->ev_pool.emplace_back(); h->ev_pool.back().create(); }
     cudaEventRecord(h->ev_pool[h->ev_used], h->stream);
     launch_merge(h, delta, 0, -1, use_xchg, batched);
     cudaEventRecord(h->ev_pool[h->ev_used + 1], h->stream);
@@ -941,15 +923,9 @@ static void filt_rebuild(bpe_handle *h, int gate_same) {
 // of the stream as it is now
 static int filt_activate(bpe_handle *h) {
     const u64 want = (u64)h->h_ctl->nseg + 64;      // segments of the stream as it is now (the count only ever falls), not the buffers' capacity
-    if (h->sig_cap < want) {
-        if (h->sig) cudaFree(h->sig);
-        if (h->cand) cudaFree(h->cand);
-        h->sig = nullptr; h->cand = nullptr; h->sig_cap = 0;
-        CU(cudaMalloc(&h->sig, want * SIG_WORDS * 4));
-        CU(cudaMalloc(&h->cand, want * 4));
-        h->sig_cap = want;
-    }
-    const u64 ptr = (u64)(uintptr_t)h->cand;
+    int rc;
+    if ((rc = dev_reserve(h, h->sig, want * SIG_WORDS)) || (rc = dev_reserve(h, h->cand, want))) return rc;
+    const u64 ptr = (u64)(uintptr_t)h->cand.p;
     const u32 zero = 0;
     CU(cudaMemcpyAsync(&h->ctl->cand_ptr, &ptr, 8, cudaMemcpyHostToDevice, h->stream));
     CU(cudaMemcpyAsync(&h->ctl->n_cand, &zero, 4, cudaMemcpyHostToDevice, h->stream));
@@ -1018,17 +994,9 @@ extern "C" int bpe_train(bpe_handle *h, int32_t num_merges, int32_t first_idx, i
     if ((u64)h->max_id + 1 >= 0x7fffffffull / 2) return fail(h, BPE_ERR_ARG, "bpe_train: ids of the loaded stream are too large for the dense delta vector");
     const u32 V = std::max(std::max((u32)first_idx + (u32)num_merges, h->max_id + 1), h->opt_vocab_cap);
     h->batching = !h->opt_rescan && batch_fits(V);
-    if ((rc = ensure_delta(h, V, h->batching ? BATCH_MAX : 1))) return rc;
-    if (h->log_cap < num_merges) {
-        if (h->log_pairs) cudaFree(h->log_pairs);
-        if (h->log_counts) cudaFree(h->log_counts);
-        h->log_pairs = nullptr; h->log_counts = nullptr; h->log_cap = 0;
-        CU(cudaMalloc(&h->log_pairs, (size_t)num_merges * 8));
-        CU(cudaMalloc(&h->log_counts, (size_t)num_merges * 8));
-        h->log_cap = num_merges;
-    }
-    cudaEvent_t ev0, ev1, ev2;
-    CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1)); CU(cudaEventCreate(&ev2));
+    if ((rc = ensure_delta(h, V, h->batching ? BATCH_MAX : 1)) || (rc = ensure_log(h, num_merges))) return rc;
+    Event ev0, ev1, ev2;
+    CU(ev0.create()); CU(ev1.create()); CU(ev2.create());
 
     // ---- initial statistics (the only full histogram of the run) ----
     CU(cudaEventRecord(ev0, h->stream));
@@ -1086,7 +1054,6 @@ extern "C" int bpe_train(bpe_handle *h, int32_t num_merges, int32_t first_idx, i
     float ms01 = 0, ms12 = 0;
     cudaEventElapsedTime(&ms01, ev0, ev1);
     cudaEventElapsedTime(&ms12, ev1, ev2);
-    cudaEventDestroy(ev0); cudaEventDestroy(ev1); cudaEventDestroy(ev2);
     h->tm.init_ms = ms01; h->tm.loop_ms = ms12;
     h->tm.tokens_in = h->h_ctl->sum_in; h->tm.tokens_out = h->h_ctl->sum_out;
     h->tm.table_slots = h->table.mask + 1; h->tm.table_used = h->h_ctl->table_used;
@@ -1132,3 +1099,8 @@ extern "C" int bpe_debug_table(bpe_handle *h, int32_t *pairs, int64_t *counts, u
 #include "encode2_host.inl"
 #include "decode_host.inl"
 #include "dedup_host.inl"
+
+bpe_handle::~bpe_handle() {   // the members free the device buffers, events and sub-states
+    if (h_ctl) cudaFreeHost(h_ctl);
+    if (own_stream) cudaStreamDestroy(own_stream);
+}

@@ -378,18 +378,34 @@ void launch(const LaunchCfg &cfg, const char *kernel, const void *func, const st
 }
 
 // ---- guarded device allocator -------------------------------------------------------------------------------------
-struct Alloc { void *base; size_t total; };
+struct Alloc { void *base; size_t total, user; };   // total == 0: posix_memalign (EMU_GUARD=0)
 static std::mutex g_mu;
 static std::map<void *, Alloc> g_allocs;
+// accounting (emu_alloc_stats): live bytes of the user sizes, their peak, cudaMalloc calls, the armed failure (emu_fail_alloc)
+static size_t g_live_bytes = 0, g_peak_bytes = 0;
+static unsigned long long g_mallocs = 0, g_fail_at = 0;
 static bool guard_on() { static int v = -1; if (v < 0) { const char *e = getenv("EMU_GUARD"); v = !(e && e[0] == '0'); } return v != 0; }
+
+static void account(void *q, const Alloc &a) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    g_allocs[q] = a;
+    g_live_bytes += a.user;
+    if (g_live_bytes > g_peak_bytes) g_peak_bytes = g_live_bytes;
+}
 
 cudaError_t dev_malloc(void **p, size_t n) {
     const size_t page = 4096;
     const size_t user = (n + 255) & ~(size_t)255;   // cudaMalloc granularity seen by the kernels: 256 B
+    {
+        std::lock_guard<std::mutex> lk(g_mu);
+        ++g_mallocs;
+        if (g_fail_at && g_mallocs == g_fail_at) { g_fail_at = 0; return cudaErrorMemoryAllocation; }
+    }
     if (!guard_on()) {
         void *q = nullptr;
         if (posix_memalign(&q, 256, user ? user : 256)) return cudaErrorMemoryAllocation;
         memset(q, 0xCD, user ? user : 256);
+        account(q, Alloc{q, 0, user});
         *p = q;
         return cudaSuccess;
     }
@@ -400,17 +416,13 @@ cudaError_t dev_malloc(void **p, size_t n) {
     mprotect(base + body, page, PROT_NONE);          // an access past the end of the allocation faults
     char *q = base + (body - user);
     if (user <= (64u << 20)) memset(q, 0xCD, user);  // never-written memory is recognisable (large buffers stay lazy)
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        g_allocs[q] = Alloc{base, total};
-    }
+    account(q, Alloc{base, total, user});
     *p = q;
     return cudaSuccess;
 }
 
 cudaError_t dev_free(void *p) {
     if (!p) return cudaSuccess;
-    if (!guard_on()) { free(p); return cudaSuccess; }
     Alloc a;
     {
         std::lock_guard<std::mutex> lk(g_mu);
@@ -418,8 +430,10 @@ cudaError_t dev_free(void *p) {
         if (it == g_allocs.end()) { fprintf(stderr, "emu: cudaFree of an unknown pointer %p\n", p); abort(); }
         a = it->second;
         g_allocs.erase(it);
+        g_live_bytes -= a.user;
     }
-    munmap(a.base, a.total);
+    if (a.total) munmap(a.base, a.total);
+    else free(p);
     return cudaSuccess;
 }
 
@@ -438,8 +452,9 @@ cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
 }
 struct emu_event { double t; };
 static double now_ms() { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec / 1e6; }
-cudaError_t cudaEventCreate(cudaEvent_t *e) { *e = new emu_event{0}; return cudaSuccess; }
-cudaError_t cudaEventDestroy(cudaEvent_t e) { delete e; return cudaSuccess; }
+static std::atomic<long long> g_live_events{0};
+cudaError_t cudaEventCreate(cudaEvent_t *e) { *e = new emu_event{0}; ++g_live_events; return cudaSuccess; }
+cudaError_t cudaEventDestroy(cudaEvent_t e) { delete e; --g_live_events; return cudaSuccess; }
 cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t) { e->t = now_ms(); return cudaSuccess; }
 cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t a, cudaEvent_t b) { *ms = (float)(b->t - a->t); return cudaSuccess; }
 
@@ -450,4 +465,16 @@ extern "C" size_t emu_kernel_trace(char *buf, size_t cap) {
     emu::g_trace.clear();
     if (cap) { const size_t n = out.size() < cap - 1 ? out.size() : cap - 1; memcpy(buf, out.data(), n); buf[n] = 0; }
     return out.size();
+}
+
+extern "C" void emu_alloc_stats(unsigned long long out[5]) {
+    std::lock_guard<std::mutex> lk(emu::g_mu);
+    out[0] = emu::g_allocs.size(); out[1] = emu::g_live_bytes; out[2] = emu::g_peak_bytes; out[3] = (unsigned long long)g_live_events.load();
+    out[4] = emu::g_mallocs;
+    emu::g_peak_bytes = emu::g_live_bytes;
+}
+
+extern "C" void emu_fail_alloc(unsigned long long k) {
+    std::lock_guard<std::mutex> lk(emu::g_mu);
+    emu::g_fail_at = k ? emu::g_mallocs + k : 0;
 }

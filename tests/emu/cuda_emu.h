@@ -76,6 +76,11 @@ void set_max_dyn_smem(const void *func, int bytes);   // cudaFuncSetAttribute(Ma
 }  // namespace emu
 // names of the kernels launched by this process since the last call, one per line (tests/emu/kernel_coverage.py)
 extern "C" size_t emu_kernel_trace(char *buf, size_t cap);
+// device-memory accounting (tests/test_emu_ownership.py): out[0] live allocations, [1] their bytes, [2] peak live bytes since
+// the last call (it restarts at the live bytes), [3] live events, [4] cudaMalloc calls so far
+extern "C" void emu_alloc_stats(unsigned long long out[5]);
+// the k-th cudaMalloc from now returns cudaErrorMemoryAllocation (k = 0: none)
+extern "C" void emu_fail_alloc(unsigned long long k);
 #define threadIdx (emu::ctx()->tid)
 #define blockIdx (emu::ctx()->bid)
 #define blockDim (emu::ctx()->bdim)
