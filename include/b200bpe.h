@@ -200,6 +200,20 @@ int bpe_encode_text_gpt4_special(bpe_handle *h, const uint8_t *bytes, uint64_t n
                                  const uint8_t *byte_perm, const uint8_t *special_bytes, const uint32_t *special_offsets,
                                  const int32_t *special_ids, int32_t n_special, int32_t *out_ids, uint64_t out_cap,
                                  uint64_t *out_n);
+/* [RegexTokenizer.encode(t, allowed_special) for t in texts] (regex.py:111-164 per document) in one call.  The documents'
+ * utf-8 bytes back to back, doc_offsets[n_docs] as bpe_dedup_add_docs validates them (empty documents allowed); every
+ * document is split on its own with BPE_OPT_SPLIT_PATTERN (needs bpe_gpt4_tables), so no chunk spans two documents, and
+ * a special token only matches inside a document.  Specials as bpe_encode_text_gpt4_special takes them; n_special = 0:
+ * encode_ordinary.  n_merges == 0 gives the bytes (their byte_perm images).  Ids of all documents go to out_ids (n ids
+ * always suffice; BPE_ERR_CAPACITY otherwise); out_doc_offsets[n_docs + 1]: document j's ids are
+ * out_ids[out_doc_offsets[j] .. out_doc_offsets[j+1]), *out_n = all ids.  Pieces of BPE_OPT_SPLIT_PIECE bytes: whole
+ * documents while they fit, a longer document cut at letter+space points.  Same memo as bpe_encode_text_gpt4 (warm across
+ * calls with the same merges), same bpe_encode_stats; a stream loaded for training and an open counting session are not
+ * disturbed. */
+int bpe_encode_docs(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *doc_offsets, uint64_t n_docs,
+                    const int32_t *merges, int32_t n_merges, const uint8_t *byte_perm,
+                    const uint8_t *special_bytes, const uint32_t *special_offsets, const int32_t *special_ids, int32_t n_special,
+                    int32_t *out_ids, uint64_t out_cap, uint64_t *out_doc_offsets, uint64_t *out_n);
 /* Counters of the memoised encode: out[0] distinct chunks in the memo table, [1] ids in its pool; of the last call:
  * [2] chunks newly added, [3] chunks encoded directly (no room in the table, or longer than 48 bytes), [4] of which
  * long, [5] pieces, [6] pieces that took the general path, [7] device microseconds of the encode kernels

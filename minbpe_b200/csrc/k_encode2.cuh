@@ -16,7 +16,8 @@
 //                   chunk's bytes with the slot's, so a tag collision can never produce a wrong id: such a chunk
 //                   is simply not found and falls to the position map / the failure flag)
 //   (scan of the tile counts: k_flag_scan_parts)
-//   k_enc_write     per tile: lookups again, ids staged in shared memory, coalesced stores to the output
+//   k_enc_write     per tile: lookups again, ids staged in shared memory, coalesced stores to the output; <true>: also
+//                   the output position of every document's first id (bpe_encode_docs, DESIGN.md §16)
 //
 // The memo table, the id pool and the rank table stay with the handle: further pieces of a long text, and later
 // encode() calls with the same merges, start warm.
@@ -494,7 +495,11 @@ __global__ void __launch_bounds__(E2_THREADS) k_enc_count(Enc2 E, u32 *__restric
 }
 
 // ---- pass 5: write the ids ------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(E2_THREADS) k_enc_write(Enc2 E, const u64 *__restrict__ excl, int *__restrict__ out) {
+// DOCS (bpe_encode_docs): the piece holds nd documents starting at dstart[] (ascending, each one a chunk start); the
+// output position of the first id of every document goes to dpos[its index]
+template <bool DOCS>
+__global__ void __launch_bounds__(E2_THREADS) k_enc_write(Enc2 E, const u64 *__restrict__ excl, int *__restrict__ out,
+                                                          const u64 *__restrict__ dstart, u32 nd, u64 *__restrict__ dpos) {
     __shared__ __align__(16) unsigned char s_b[E2_TILE + E2_HALO + 8];
     __shared__ u32 s_bits[(E2_TILE + E2_HALO) / 32 + 2];
     __shared__ u32 s_scan[E2_THREADS / 32];
@@ -530,6 +535,21 @@ __global__ void __launch_bounds__(E2_THREADS) k_enc_write(Enc2 E, const u64 *__r
 #pragma unroll
     for (int w = 0; w < E2_THREADS / 32; ++w) { const u32 v = s_scan[w]; if ((u32)w < warp) wbase += v; total += v; }
     u32 dst = wbase + incl - sum;
+    if constexpr (DOCS) {
+        if (cnt) {   // the first document start at or after this thread's bytes (one binary search), then a walk
+            const u64 p0 = lo + base;
+            u32 a = 0, b = nd;
+            while (a < b) { const u32 mid = (a + b) >> 1; if (dstart[mid] < p0) a = mid + 1; else b = mid; }
+            u32 mine2 = bits, d = dst;
+            for (u32 c = 0; c < cnt && a < nd; ++c) {
+                const u64 p = lo + base + (__ffs(mine2) - 1);
+                mine2 &= mine2 - 1;
+                while (a < nd && dstart[a] < p) ++a;      // none: every document start is a chunk start (the host checks)
+                if (a < nd && dstart[a] == p) { dpos[a] = excl[blockIdx.x] + d; ++a; }
+                d += nts[c];
+            }
+        }
+    }
     int *o = out + excl[blockIdx.x];
     for (u32 c = 0; c < cnt; ++c) {
         const u32 nt = nts[c], off = offs[c];

@@ -6,7 +6,8 @@
 //   k_special_find    every text position where some special starts -> (position, lowest matching index), appended to a
 //                     list (specials are rare; the host sorts the list and drops overlapped candidates left to right)
 //   k_special_meta    bytes of the accepted occurrences get the boundary class SC_B in the splitter's class array, so
-//                     the GPT-4 split treats the text on either side as separate texts (split_logic.h, WITH_B)
+//                     the GPT-4 split treats the text on either side as separate texts (split_logic.h, WITH_B);
+//                     <true> also marks them SM_SPEC (a split buffer of documents, DESIGN.md §16)
 //   k_special_flags   chunk-start flags: one chunk per occurrence, and a chunk start right behind it
 // The memoised encode (k_encode2.cuh) then needs nothing new: the specials are seeded into the memo table as chunks
 // whose "encoding" is their single id (k_enc_seed_specials).
@@ -47,12 +48,15 @@ __global__ void __launch_bounds__(256) k_special_find(const unsigned char *__res
     }
 }
 
-// accepted occurrences: hit[j] = position << 8 | length
+// accepted occurrences: hit[j] = position << 8 | length.  DOCS: a split buffer of documents (bpe_encode_docs), whose gaps
+// have class SC_B as well: the occurrence's bytes also get SM_SPEC, so that the compaction (k_flag_reduce / k_flag_scatter
+// <true, true>) tells them apart from the gaps
+template <bool DOCS>
 __global__ void k_special_meta(unsigned char *__restrict__ meta, const u64 *__restrict__ hit, u64 m) {
     for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < m; j += (u64)gridDim.x * blockDim.x) {
         const u64 pos = hit[j] >> 8;
         const u32 len = (u32)(hit[j] & 0xffu);
-        for (u32 t = 0; t < len; ++t) meta[pos + t] = (unsigned char)((meta[pos + t] & SM_START) | SC_B);
+        for (u32 t = 0; t < len; ++t) meta[pos + t] = (unsigned char)((meta[pos + t] & SM_START) | SC_B | (DOCS ? SM_SPEC : 0u));
     }
 }
 

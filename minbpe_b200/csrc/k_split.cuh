@@ -62,11 +62,17 @@ __device__ __forceinline__ u32 gaps_before(const u64 *__restrict__ doff, u32 nd,
     }
     return lo;
 }
-__device__ __forceinline__ bool is_gap(const unsigned char *__restrict__ meta, u64 p) { return (meta[p] & SM_CLS) == SC_B; }
+// SPEC: the buffer also holds special-token occurrences (bpe_encode_docs), class SC_B with SM_SPEC (k_special_meta<true>);
+// they are not gaps
+template <bool SPEC = false>
+__device__ __forceinline__ bool is_gap(const unsigned char *__restrict__ meta, u64 p) {
+    return SPEC ? (meta[p] & (SM_CLS | SM_SPEC)) == SC_B : (meta[p] & SM_CLS) == SC_B;
+}
 // chunk start at position p of the split buffer of documents: not a boundary byte, and a flag of the rule or the first
 // byte of a document (the boundary's own one-byte chunk is dropped)
+template <bool SPEC = false>
 __device__ __forceinline__ u32 doc_chunk_start(const unsigned char *__restrict__ flag, const unsigned char *__restrict__ meta, u64 p) {
-    return !is_gap(meta, p) && (flag[p] || (p > 0 && is_gap(meta, p - 1))) ? 1u : 0u;
+    return !is_gap<SPEC>(meta, p) && (flag[p] || (p > 0 && is_gap<SPEC>(meta, p - 1))) ? 1u : 0u;
 }
 
 // meta[i] = class of the character byte i belongs to | SM_START on its first byte.
@@ -266,15 +272,16 @@ __global__ void __launch_bounds__(256) k_widen_marked(const unsigned char *__res
 
 // ---- flag compaction: chunk offsets (3-kernel sum scan over the same tiles) ----
 // DOCS: flags of a split buffer of documents (k_split_classify<true>): the chunk starts are doc_chunk_start's, and
-// k_flag_scatter<true> writes them at their positions in the documents' own bytes (the boundary bytes taken out)
-template <bool DOCS>
+// k_flag_scatter<true> writes them at their positions in the documents' own bytes (the boundary bytes taken out).  SPEC
+// (with DOCS): the documents hold special-token occurrences, which stay (is_gap<true>)
+template <bool DOCS, bool SPEC = false>
 __global__ void __launch_bounds__(SP_THREADS) k_flag_reduce(const unsigned char *__restrict__ flag, u64 n, u32 *__restrict__ part,
                                                             const unsigned char *__restrict__ meta) {
     __shared__ u32 sm[SP_THREADS];
     const u64 base = (u64)blockIdx.x * SP_TILE + (u64)threadIdx.x * SP_ITEMS;
     u32 c = 0;
 #pragma unroll
-    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += DOCS ? doc_chunk_start(flag, meta, base + k) : flag[base + k];
+    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += DOCS ? doc_chunk_start<SPEC>(flag, meta, base + k) : flag[base + k];
     sm[threadIdx.x] = c;
     __syncthreads();
     for (int o = SP_THREADS / 2; o > 0; o >>= 1) { if (threadIdx.x < (u32)o) sm[threadIdx.x] += sm[threadIdx.x + o]; __syncthreads(); }
@@ -297,7 +304,7 @@ __global__ void __launch_bounds__(1024) k_flag_scan_parts(const u32 *__restrict_
 }
 
 // offs[] = text_base + position of every set flag (text_base: where this piece starts in the caller's text)
-template <bool DOCS>
+template <bool DOCS, bool SPEC = false>
 __global__ void __launch_bounds__(SP_THREADS) k_flag_scatter(const unsigned char *__restrict__ flag, u64 n, const u64 *__restrict__ excl,
                                                              u64 *__restrict__ offs, u64 text_base, const unsigned char *__restrict__ meta,
                                                              const u64 *__restrict__ doff, u32 nd) {
@@ -306,7 +313,7 @@ __global__ void __launch_bounds__(SP_THREADS) k_flag_scatter(const unsigned char
     const u64 base = (u64)blockIdx.x * SP_TILE + (u64)tid * SP_ITEMS;
     u32 c = 0;
 #pragma unroll
-    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += DOCS ? doc_chunk_start(flag, meta, base + k) : flag[base + k];
+    for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) c += DOCS ? doc_chunk_start<SPEC>(flag, meta, base + k) : flag[base + k];
     sm[tid] = c;
     __syncthreads();
     for (int o = 1; o < SP_THREADS; o <<= 1) { const u32 v = tid >= (u32)o ? sm[tid - o] : 0; __syncthreads(); sm[tid] += v; __syncthreads(); }
@@ -317,8 +324,8 @@ __global__ void __launch_bounds__(SP_THREADS) k_flag_scatter(const unsigned char
     } else if (c) {
         u64 gaps = gaps_before(doff, nd, base);
         for (int k = 0; k < SP_ITEMS && base + k < n; ++k) {
-            if (is_gap(meta, base + k)) ++gaps;
-            else if (doc_chunk_start(flag, meta, base + k)) offs[dst++] = text_base + base + k - gaps;
+            if (is_gap<SPEC>(meta, base + k)) ++gaps;
+            else if (doc_chunk_start<SPEC>(flag, meta, base + k)) offs[dst++] = text_base + base + k - gaps;
         }
     }
 }

@@ -27,6 +27,8 @@
                    // WITH_B instantiations of the functions below know this class; the plain GPT-4 split never produces it.
 #define SM_CLS 7u
 #define SM_START 8u     // meta bit: first byte of a UTF-8 sequence
+#define SM_SPEC 16u     // meta bit: byte of a special-token occurrence in a split buffer of documents (k_special_meta<true>), which
+                        // tells it apart from a document gap (also SC_B); the rule below never reads it
 #define SPL_PK_NONE 7u  // "kind of the character in front of the run" at the start of the text
 
 // run kind: letters, digits, whitespace (SP or NL), other (O or apostrophe)

@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
 OPT_DEDUP_LOG2 = 11
@@ -70,6 +70,7 @@ def load_library():
         "bpe_encode": ([vp, vp, u64, vp, u64, vp, i32, vp, vp, u64, P(u64)], ci),
         "bpe_encode_text_gpt4": ([vp, vp, u64, vp, i32, vp, vp, u64, P(u64)], ci),
         "bpe_encode_text_gpt4_special": ([vp, vp, u64, vp, i32, vp, vp, vp, vp, i32, vp, u64, P(u64)], ci),
+        "bpe_encode_docs": ([vp, vp, u64, vp, u64, vp, i32, vp, vp, vp, vp, i32, vp, u64, vp, P(u64)], ci),
         "bpe_encode_stats": ([vp, vp], ci),
         "bpe_get_timing": ([vp, P(Timing)], ci),
         "bpe_set_option": ([vp, ci, i64], ci),
@@ -303,10 +304,7 @@ class Engine:
             out = np.empty(max(b.size, 1), dtype=np.int32)
         n = ctypes.c_uint64()
         if specials:
-            blob = np.frombuffer(b"".join(t for t, _ in specials), dtype=np.uint8)
-            offs = np.zeros(len(specials) + 1, dtype=np.uint32)
-            np.cumsum([len(t) for t, _ in specials], out=offs[1:])
-            ids = np.asarray([i for _, i in specials], dtype=np.int32)
+            blob, offs, ids = self._specials(specials)
             self._check(self._lib.bpe_encode_text_gpt4_special(
                 self._h, _ptr(b) if b.size else None, b.size, _ptr(m) if m.size else None, m.shape[0], _ptr(perm),
                 _ptr(blob), _ptr(offs), _ptr(ids), len(specials), _ptr(out), out.size, ctypes.byref(n)), "bpe_encode_text_gpt4_special")
@@ -314,6 +312,34 @@ class Engine:
         self._check(self._lib.bpe_encode_text_gpt4(self._h, _ptr(b) if b.size else None, b.size, _ptr(m) if m.size else None,
                                                    m.shape[0], _ptr(perm), _ptr(out), out.size, ctypes.byref(n)), "bpe_encode_text_gpt4")
         return out[: n.value]
+
+    @staticmethod
+    def _specials(specials):
+        """[(utf-8 bytes, id), ...] -> (bytes, offsets uint32[k+1], ids int32) of the special-token arguments."""
+        blob = np.frombuffer(b"".join(t for t, _ in specials), dtype=np.uint8)
+        offs = np.zeros(len(specials) + 1, dtype=np.uint32)
+        np.cumsum([len(t) for t, _ in specials], out=offs[1:])
+        return blob, offs, np.asarray([i for _, i in specials], dtype=np.int32)
+
+    def encode_docs(self, data, doc_offsets, merges, byte_perm=None, specials=None):
+        """Many documents in one call (bpe_encode_docs): `data` = their utf-8 bytes back to back, doc_offsets = the start of
+        every document.  Every document is split on its own (BPE_OPT_SPLIT_PATTERN) and encoded as encode_text_gpt4 would
+        encode it alone, specials included.  -> (ids int32 of all documents, uint64[n_docs + 1]: document j's ids are
+        ids[o[j]:o[j+1]])."""
+        self._ensure_gpt4_tables()
+        b = _u8(data)
+        o = np.ascontiguousarray(doc_offsets, dtype=np.uint64)
+        m = np.ascontiguousarray(np.asarray(merges, dtype=np.int32).reshape(-1, 2))
+        perm = None if byte_perm is None else np.ascontiguousarray(byte_perm, dtype=np.uint8)
+        out = np.empty(max(b.size, 1), dtype=np.int32)
+        out_offs = np.empty(o.size + 1, dtype=np.uint64)
+        blob, soffs, sids = self._specials(specials) if specials else (None, None, None)
+        n = ctypes.c_uint64()
+        self._check(self._lib.bpe_encode_docs(
+            self._h, _ptr(b) if b.size else None, b.size, _ptr(o) if o.size else None, o.size, _ptr(m) if m.size else None,
+            m.shape[0], _ptr(perm), _ptr(blob), _ptr(soffs), _ptr(sids), len(specials) if specials else 0, _ptr(out), out.size,
+            _ptr(out_offs), ctypes.byref(n)), "bpe_encode_docs")
+        return out[: n.value], out_offs
 
     def encode_stats(self):
         a = np.zeros(10, dtype=np.uint64)

@@ -571,3 +571,59 @@ class RegexTokenizer(Tokenizer):
             else:
                 ids.extend(self.encode_ordinary(part))
         return ids
+
+    def encode_ordinary_batch(self, texts):
+        """[self.encode_ordinary(t) for t in texts], not in the reference (tiktoken has it): many documents in few device calls."""
+        return self._encode_batch(texts, None)
+
+    def encode_batch(self, texts, allowed_special="none_raise"):
+        """[self.encode(t, allowed_special) for t in texts], errors included, not in the reference (tiktoken and HF
+        `tokenizers` have it).  For the GPT-2 / GPT-4 patterns and batches of at least DEVICE_SPLIT_MIN_BYTES the documents
+        go to the GPU in batches of ITERATOR_BATCH_BYTES (bpe_encode_docs): every document is split on its own there, its
+        special tokens found inside it only, and every distinct chunk encoded once through the memo.  Anything else is the
+        per-document loop."""
+        return self._encode_batch(texts, allowed_special)
+
+    def _encode_batch(self, texts, allowed_special):
+        texts = list(texts)
+        if not texts:
+            return []
+        if allowed_special is None or allowed_special == "none" or allowed_special == "none_raise":
+            special = {}
+        elif allowed_special == "all":
+            special = self.special_tokens
+        elif isinstance(allowed_special, set):
+            special = {k: v for k, v in self.special_tokens.items() if k in allowed_special}
+        else:
+            raise ValueError(f"allowed_special={allowed_special} not understood")
+        data = []
+        for t in texts:        # before any device work, in document order
+            if not isinstance(t, str):
+                raise TypeError(f"encode_batch takes str documents, got {type(t).__name__}")
+            if allowed_special == "none_raise":
+                assert all(token not in t for token in self.special_tokens)
+            data.append(t.encode("utf-8"))
+        which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
+        if (which is None or not self.merges or sum(map(len, data)) < self.DEVICE_SPLIT_MIN_BYTES or
+                (special and not self._device_specials(special))):
+            if allowed_special is None:
+                return [self.encode_ordinary(t) for t in texts]
+            return [self.encode(t, allowed_special) for t in texts]
+        from .engine import OPT_SPLIT_PATTERN
+        eng = self.engine
+        eng.set_option(OPT_SPLIT_PATTERN, which)
+        merges = self._merge_array()
+        spec = [(k.encode("utf-8"), int(v)) for k, v in special.items()] or None
+        out, j = [], 0
+        while j < len(data):   # batches of at least ITERATOR_BATCH_BYTES (or the rest), as train_from_iterator sends them
+            k, size = j, 0
+            while k < len(data) and size < self.ITERATOR_BATCH_BYTES:
+                size += len(data[k])
+                k += 1
+            offs = np.zeros(k - j, dtype=np.uint64)
+            if k - j > 1:
+                np.cumsum([len(b) for b in data[j: k - 1]], out=offs[1:])
+            ids, o = eng.encode_docs(b"".join(data[j:k]), offs, merges, self._byte_perm, spec)
+            out.extend(a.tolist() for a in np.split(ids, o[1:-1].astype(np.int64)))
+            j = k
+        return out
