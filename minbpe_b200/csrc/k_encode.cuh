@@ -5,7 +5,8 @@
 //
 // Chunks are independent and tiny (mean ~5 bytes for the GPT-4 split), so the natural mapping is
 //   k_encode_chunks  one THREAD per chunk (<= ENC_LOCAL tokens), tokens in a per-thread array,
-//                    merge ranks from an open-addressing table that lives in L2/L1
+//                    merge ranks from an open-addressing table that lives in L2/L1 (encode_chunk_thread, which
+//                    the memoised path's one-thread kernels run as well)
 //   k_encode_long    one CTA per long chunk (<= ENC_LONG_MAX tokens), tokens in shared memory
 // Ids are written at the chunk's own byte offset in a buffer of n words, unused tail slots get
 // ENC_HOLE; k_compact_holes then squeezes every 512-word segment in place and leaves segment
@@ -56,6 +57,26 @@ __global__ void k_rank_table_build(const int *__restrict__ merges, int n_merges,
     atomicMax(&ranks[slot], (u32)r);
 }
 
+// regex.py:92-109 on a short token list held by one thread: tok[0, len) in/out, returns the new length
+__device__ __forceinline__ u32 encode_chunk_thread(u32 *tok, u32 len, const RankTable &rt) {
+    while (len >= 2) {
+        u32 best = RANK_NONE, ba = 0, bb = 0;
+        for (u32 i = 0; i + 1 < len; ++i) {
+            const u32 r = rank_of(rt, tok[i], tok[i + 1]);
+            if (r < best) { best = r; ba = tok[i]; bb = tok[i + 1]; }
+        }
+        if (best == RANK_NONE) break;
+        const u32 z = 256u + best;
+        u32 j = 0;
+        for (u32 i = 0; i < len;) {
+            if (i + 1 < len && tok[i] == ba && tok[i + 1] == bb) { tok[j++] = z; i += 2; }
+            else tok[j++] = tok[i++];
+        }
+        len = j;
+    }
+    return len;
+}
+
 __global__ void __launch_bounds__(128) k_encode_chunks(const unsigned char *__restrict__ bytes, const u64 *__restrict__ offs,
                                                        u64 n_chunks, u64 n, RankTable rt,
                                                        const unsigned char *__restrict__ perm, u32 *__restrict__ out,
@@ -75,22 +96,7 @@ __global__ void __launch_bounds__(128) k_encode_chunks(const unsigned char *__re
         const u32 b = bytes[lo + i];
         tok[i] = perm ? perm[b] : b;
     }
-    u32 len = len0;
-    while (len >= 2) {
-        u32 best = RANK_NONE, ba = 0, bb = 0;
-        for (u32 i = 0; i + 1 < len; ++i) {
-            const u32 r = rank_of(rt, tok[i], tok[i + 1]);
-            if (r < best) { best = r; ba = tok[i]; bb = tok[i + 1]; }
-        }
-        if (best == RANK_NONE) break;
-        const u32 z = 256u + best;
-        u32 j = 0;
-        for (u32 i = 0; i < len;) {
-            if (i + 1 < len && tok[i] == ba && tok[i + 1] == bb) { tok[j++] = z; i += 2; }
-            else tok[j++] = tok[i++];
-        }
-        len = j;
-    }
+    const u32 len = encode_chunk_thread(tok, len0, rt);
     for (u32 i = 0; i < len0; ++i) out[lo + i] = (i < len) ? tok[i] : ENC_HOLE;
 }
 

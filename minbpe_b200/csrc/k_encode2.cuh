@@ -252,26 +252,6 @@ __global__ void k_enc_seed_specials(Enc2 E, const unsigned char *__restrict__ bl
     atomicOr(&E.ctl->fail, E2_FAIL_OTHER);
 }
 
-// regex.py:92-109 on a short token list held by one thread.  tok[] in/out, returns the new length.
-__device__ __forceinline__ u32 e2_encode_short(u32 *tok, u32 len, const RankTable &rt) {
-    while (len >= 2) {
-        u32 best = RANK_NONE, ba = 0, bb = 0;
-        for (u32 i = 0; i + 1 < len; ++i) {
-            const u32 r = rank_of(rt, tok[i], tok[i + 1]);
-            if (r < best) { best = r; ba = tok[i]; bb = tok[i + 1]; }
-        }
-        if (best == RANK_NONE) break;
-        const u32 z = 256u + best;
-        u32 j = 0;
-        for (u32 i = 0; i < len;) {
-            if (i + 1 < len && tok[i] == ba && tok[i + 1] == bb) { tok[j++] = z; i += 2; }
-            else tok[j++] = tok[i++];
-        }
-        len = j;
-    }
-    return len;
-}
-
 // ---- pass 2: encode every newly claimed slot once ------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_enc_distinct(Enc2 E, RankTable rt, const unsigned char *__restrict__ perm) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -284,7 +264,7 @@ __global__ void __launch_bounds__(128) k_enc_distinct(Enc2 E, RankTable rt, cons
         const u32 b = (m->key[k >> 2] >> (8u * (k & 3u))) & 0xffu;
         tok[k] = perm ? perm[b] : b;
     }
-    const u32 len = e2_encode_short(tok, len0, rt);
+    const u32 len = encode_chunk_thread(tok, len0, rt);
     const ull off = atomicAdd(&E.ctl->pool_used, (ull)len);
     if (off + len > E.pool_cap) { atomicOr(&E.ctl->fail, E2_FAIL_OTHER); return; }
     for (u32 k = 0; k < len; ++k) E.pool[off + k] = tok[k];
@@ -318,7 +298,7 @@ __global__ void __launch_bounds__(128) k_enc_direct_short(Enc2 E, RankTable rt, 
         const u32 b = E.text[q];
         tok[len0++] = perm ? perm[b] : b;
     }
-    const u32 len = e2_encode_short(tok, len0, rt);
+    const u32 len = encode_chunk_thread(tok, len0, rt);
     const ull off = atomicAdd(&E.ctl->tmp_used, (ull)len);
     if (off + len > E.tmp_cap) { atomicOr(&E.ctl->fail, E2_FAIL_TMP); return; }
     for (u32 k = 0; k < len; ++k) E.tmp[off + k] = tok[k];
