@@ -229,6 +229,10 @@ int bpe_encode_stats(bpe_handle *h, uint64_t *out /* [10] */);
  * 4 apostrophe, 5 other} for cp < 0x110000, contr_table[cp] (cp < 0x3000) = bit0 (?i:[sdmt]),
  * bit1 (?i:l), bit2 (?i:v), bit3 (?i:e), bit4 (?i:r). */
 int bpe_gpt4_tables(bpe_handle *h, const uint8_t *cls_table, const uint8_t *contr_table);
+/* The table of the o200k split pattern (BPE_OPT_SPLIT_PATTERN 3), after bpe_gpt4_tables: case_table[cp] in {0 none,
+ * 1 \p{Lu} or \p{Lt}, 2 \p{Ll}, 3 \p{Lm} or \p{Lo}, 4 \p{M}} for cp < 0x110000 (minbpe_b200/unicode_tables.py
+ * o200k_table).  '/' is recognised from its byte; contractions use contr_table. */
+int bpe_o200k_table(bpe_handle *h, const uint8_t *case_table);
 /* Chunk start offsets (bytes) of valid UTF-8 `bytes` under the GPT-4 pattern.  Any length: texts beyond 1 GiB are
  * processed in pieces cut at provable chunk boundaries (ASCII letter followed by U+0020). */
 int bpe_split_gpt4(bpe_handle *h, const uint8_t *bytes, uint64_t n, uint64_t *out_offsets, uint64_t cap,
@@ -335,8 +339,10 @@ int bpe_get_timing(bpe_handle *h, bpe_timing *out);
 #define BPE_OPT_ENC_MEMO_LOG2 7 /* test hook: log2 of the slots of the encode memo table (0 = default 22); drops the current table */
 #define BPE_OPT_SPLIT_PIECE 5   /* test hook: bytes per piece of the device splitter (0 = default 1 GiB); texts longer than
                                    a piece are cut where a letter is followed by U+0020 (process-wide) */
-#define BPE_OPT_SPLIT_PATTERN 8 /* which of the reference's two split patterns (regex.py:18-19) the *_gpt4 entry points apply:
-                                   0 = GPT4_SPLIT_PATTERN (default), 1 = GPT2_SPLIT_PATTERN; per handle */
+#define BPE_OPT_SPLIT_PATTERN 8 /* which split pattern the *_gpt4 entry points apply: 0 = GPT4_SPLIT_PATTERN (default),
+                                   1 = GPT2_SPLIT_PATTERN (the reference's two, regex.py:18-19), 3 = O200K_SPLIT_PATTERN
+                                   (tiktoken o200k_base, GPT-4o; needs bpe_o200k_table); per handle.  2 is not a pattern
+                                   and stays an error: it was rejected when only 0 and 1 existed, and callers rely on that */
 #define BPE_OPT_HIST_KERNEL 9   /* byte-pair histogram of iteration 0: 2 = k_hist_dense (default);
                                    1 = k_hist_dense_packed; 0 = k_hist_dense until the first stream of >= 8 Mi tokens, where
                                    k_hist_dense_packed is cross-checked and timed against it and adopted if equal and not slower */

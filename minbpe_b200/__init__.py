@@ -9,6 +9,7 @@ hand-written sm_90a CUDA kernels reached through the C ABI in include/b200bpe.h.
 from .tokenizer import (  # noqa: F401
     GPT2_SPLIT_PATTERN,
     GPT4_SPLIT_PATTERN,
+    O200K_SPLIT_PATTERN,
     BasicTokenizer,
     RegexTokenizer,
     Tokenizer,

@@ -28,7 +28,7 @@
 #include "k_weighted.cuh"
 #include "k_dedup.cuh"
 
-#define BPE_ABI_VERSION 5
+#define BPE_ABI_VERSION 6
 
 namespace {   // the owner types stay private to the library: they add no exported symbol
 
@@ -124,6 +124,7 @@ struct bpe_handle {
     DevBuf<Best> partials;
     DevBuf<TopList> top_partials;      // k_select_batch: one list per block
     DevBuf<unsigned char> d_cls, d_contr;   // code-point class / contraction tables of the GPT-4 splitter
+    DevBuf<unsigned char> d_cls_o200k;      // class table of the o200k split: GPT-4 class | case class << 5 (bpe_o200k_table)
     // sharded loop over NVLink peer memory (k_xchg.cuh): the rank's exchange block and its peers' mappings
     unsigned char *xchg = nullptr; u64 xchg_bytes = 0, xchg_stride = 0; u32 xchg_V = 0;
     XArgs xargs = {};
@@ -142,7 +143,7 @@ struct bpe_handle {
                                  // 0 = decide at the first large stream (cross-check + timing)
     int opt_dedup_log2 = 0;      // BPE_OPT_DEDUP_LOG2 (test hook): log2 slots of the chunk table of bpe_load_text_gpt4_dedup, 0 = default
     u64 dd_stats[8] = {};        // bpe_dedup_stats of the last bpe_load_text_gpt4_dedup / bpe_dedup_finish
-    int opt_split_pattern = 0;   // BPE_OPT_SPLIT_PATTERN: 0 = GPT-4 split pattern, 1 = GPT-2 (bpe_split_gpt4 / bpe_load_text_gpt4 / bpe_encode_text_gpt4*)
+    int opt_split_pattern = 0;   // BPE_OPT_SPLIT_PATTERN: 0 = GPT-4 split pattern, 1 = GPT-2, 3 = o200k (bpe_split_gpt4 / bpe_load_text_gpt4 / bpe_encode_text_gpt4*)
 
     bpe_timing tm = {};
     std::vector<Event> ev_pool;  // per-launch timing of the fused merge kernel (BPE_OPT_KERNEL_TIMING)
@@ -317,7 +318,7 @@ extern "C" int bpe_set_option(bpe_handle *h, int opt, int64_t value) {
             if (value == 0) h->hist_mode = 0;
             break;
         case BPE_OPT_SPLIT_PATTERN:
-            if (value != 0 && value != 1) return fail(h, BPE_ERR_ARG, "split pattern must be 0 (GPT-4) or 1 (GPT-2)");
+            if (value != 0 && value != 1 && value != 3) return fail(h, BPE_ERR_ARG, "split pattern must be 0 (GPT-4), 1 (GPT-2) or 3 (o200k)");
             h->opt_split_pattern = (int)value; break;
         case BPE_OPT_DEDUP_LOG2:
             if (value != 0 && (value < 4 || value > 30)) return fail(h, BPE_ERR_ARG, "dedup log2 must be 0 or in [4,30]");

@@ -15,6 +15,8 @@
 //   k_split_apply       per tile: both scans in shared memory seeded with the carries, the rule per
 //                       character, and either the flag byte (offsets for encode / host callers) or the
 //                       token word with the chunk mark (training: no offsets array, no flag array)
+//   <…, 3>              the o200k pattern on its own scans: k_split_reduce<WITH_B, 3> (aggregates and their
+//                       prefixes in one launch) and k_split_apply<TOKENS, WITH_B, 3> (DESIGN.md §17)
 // Nothing per byte is materialised in HBM except the 1-byte class array.
 #pragma once
 #include "common.cuh"
@@ -180,13 +182,168 @@ __global__ void __launch_bounds__(1024) k_split_scan_parts(SplFwd *__restrict__ 
     for (u32 t = hi; t > lo; --t) { const SplBwd x = bpart[t - 1]; bpart[t - 1] = grun; grun = spl_bwd_combine(x, grun); }
 }
 
+// ---- the o200k pattern (BPE_OPT_SPLIT_PATTERN 3): its own scans (split_logic.h: SplFwdO, the automaton maps, and SplBwdO),
+// in two kernels.  k_split_reduce<WITH_B, 3> writes the tile aggregates and, in the block that finishes last, turns them
+// into exclusive prefixes (k_split_scan_parts' work); k_split_apply<TOKENS, WITH_B, 3> runs split_apply_o200k.  The
+// forward element of a character reads up to 9 bytes ahead of it (the character that follows, a contraction), so the
+// reduce kernel reads the text too.  The aggregates live in the room of the SplFwd / SplBwd ones (same sizes).
+struct FwdOOp { __device__ __forceinline__ SplFwdO operator()(SplFwdO a, SplFwdO b) const { return spl_fwdo_combine(a, b); } };
+struct BwdOOp { __device__ __forceinline__ SplBwdO operator()(SplBwdO a, SplBwdO b) const { return spl_bwdo_combine(a, b); } };
+
+// aggregates written by other blocks of the same launch: read past L1
+__device__ __forceinline__ SplFwdO ld_fwdo(const SplFwdO *p) { SplFwdO r; r.map = *(const volatile unsigned long long *)&p->map; return r; }
+__device__ __forceinline__ SplBwdO ld_bwdo(const SplBwdO *p) {
+    SplBwdO r; r.toend = *(const volatile u32 *)&p->toend; r.bits = *(const volatile u32 *)&p->bits; return r;
+}
+
+// ticket: a zeroed counter (the host clears it before the launch)
+template <bool WITH_B, int PATTERN>
+__global__ void __launch_bounds__(SP_THREADS) k_split_reduce(const unsigned char *__restrict__ b, const unsigned char *__restrict__ meta,
+                                                             u64 n, const unsigned char *__restrict__ contr,
+                                                             SplFwdO *__restrict__ fpart, SplBwdO *__restrict__ bpart, u32 *ticket) {
+    static_assert(PATTERN == 3, "the GPT-4 and GPT-2 patterns use k_split_reduce<WITH_B> and k_split_scan_parts");
+    __shared__ SplFwdO sf[SP_THREADS];
+    __shared__ SplBwdO sb[SP_THREADS];
+    __shared__ bool last;
+    const u32 tid = threadIdx.x;
+    const GmemBytes B{b}, M{meta};
+    const u64 base = (u64)blockIdx.x * SP_TILE + (u64)tid * SP_ITEMS;
+    SplFwdO f = spl_fwdo_identity();
+    SplBwdO g = spl_bwdo_identity();
+#pragma unroll
+    for (int k = 0; k < SP_ITEMS; ++k)
+        if (base + k < n) f = spl_fwdo_combine(f, spl_fwdo_elem<WITH_B>(base + k, n, B, M, contr));
+#pragma unroll
+    for (int k = SP_ITEMS - 1; k >= 0; --k)
+        if (base + k < n) g = spl_bwdo_combine(spl_bwdo_elem<WITH_B>(base + k, n, meta[base + k], base + k + 1 < n ? meta[base + k + 1] : 0u), g);
+    f = block_reduce_ordered(f, FwdOOp(), sf, SP_THREADS);
+    g = block_reduce_ordered(g, BwdOOp(), sb, SP_THREADS);
+    if (tid == 0) {
+        fpart[blockIdx.x] = f; bpart[blockIdx.x] = g;
+        __threadfence();
+        last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    // the last block: exclusive scans of all aggregates, forward left to right, backward right to left
+    const u32 ntiles = gridDim.x, per = (ntiles + SP_THREADS - 1) / SP_THREADS;
+    const u32 lo = min(ntiles, tid * per), hi = min(ntiles, lo + per);
+    f = spl_fwdo_identity();
+    for (u32 t = lo; t < hi; ++t) f = spl_fwdo_combine(f, ld_fwdo(fpart + t));
+    g = spl_bwdo_identity();
+    for (u32 t = hi; t > lo; --t) g = spl_bwdo_combine(ld_bwdo(bpart + t - 1), g);
+    sf[tid] = f; sb[tid] = g;
+    __syncthreads();
+    for (u32 o = 1; o < SP_THREADS; o <<= 1) {   // inclusive: forward over lower tids, backward over higher tids
+        SplFwdO fv = spl_fwdo_identity(); SplBwdO gv = spl_bwdo_identity();
+        if (tid >= o) fv = sf[tid - o];
+        if (tid + o < SP_THREADS) gv = sb[tid + o];
+        __syncthreads();
+        sf[tid] = spl_fwdo_combine(fv, sf[tid]); sb[tid] = spl_bwdo_combine(sb[tid], gv);
+        __syncthreads();
+    }
+    SplFwdO frun = spl_fwdo_identity();
+    if (tid > 0) frun = sf[tid - 1];
+    for (u32 t = lo; t < hi; ++t) { const SplFwdO x = ld_fwdo(fpart + t); fpart[t] = frun; frun = spl_fwdo_combine(frun, x); }
+    SplBwdO grun = spl_bwdo_identity();
+    if (tid + 1 < SP_THREADS) grun = sb[tid + 1];
+    for (u32 t = hi; t > lo; --t) { const SplBwdO x = ld_bwdo(bpart + t - 1); bpart[t - 1] = grun; grun = spl_bwdo_combine(x, grun); }
+}
+
+// per tile of the o200k split: both scans seeded with the prefixes of k_split_reduce<WITH_B, 3>, the rule, and the outputs
+// of k_split_apply
+template <bool TOKENS, bool WITH_B>
+__device__ __forceinline__ void split_apply_o200k(const unsigned char *__restrict__ b, const unsigned char *__restrict__ meta, u64 n,
+                                                  const unsigned char *__restrict__ contr,
+                                                  const SplFwdO *__restrict__ fpart, const SplBwdO *__restrict__ bpart,
+                                                  unsigned char *__restrict__ flag, u32 *__restrict__ dst) {
+    __shared__ __align__(16) unsigned char s_b[SP_TILE + 2 * SP_HALO];
+    __shared__ __align__(16) unsigned char s_m[SP_TILE + 2 * SP_HALO];
+    __shared__ SplFwdO sf[SP_THREADS];
+    __shared__ SplBwdO sb[SP_THREADS];
+    const u32 tid = threadIdx.x;
+    const u64 lo = (u64)blockIdx.x * SP_TILE;
+    for (u32 j = tid; j < SP_TILE + 2 * SP_HALO; j += SP_THREADS) {
+        const u64 pos = lo + j;
+        const bool in = pos >= SP_HALO && pos - SP_HALO < n;
+        s_b[j] = in ? b[pos - SP_HALO] : 0;
+        s_m[j] = in ? meta[pos - SP_HALO] : 0;
+    }
+    __syncthreads();
+    const SmemBytes B{s_b + SP_HALO, lo}, M{s_m + SP_HALO, lo};
+    const u64 base = lo + (u64)tid * SP_ITEMS;
+    const unsigned char *mm = s_m + SP_HALO + tid * SP_ITEMS;
+    SplFwdO fe[SP_ITEMS]; SplBwdO ge[SP_ITEMS];
+    SplFwdO f = spl_fwdo_identity();
+    SplBwdO g = spl_bwdo_identity();
+#pragma unroll
+    for (int k = 0; k < SP_ITEMS; ++k) {
+        if (base + k < n) { fe[k] = spl_fwdo_elem<WITH_B>(base + k, n, B, M, contr); ge[k] = spl_bwdo_elem<WITH_B>(base + k, n, mm[k], mm[k + 1]); }
+        else { fe[k] = spl_fwdo_identity(); ge[k] = spl_bwdo_identity(); }
+        f = spl_fwdo_combine(f, fe[k]);
+    }
+#pragma unroll
+    for (int k = SP_ITEMS - 1; k >= 0; --k) g = spl_bwdo_combine(ge[k], g);
+    sf[tid] = f; sb[tid] = g;
+    __syncthreads();
+    for (u32 o = 1; o < SP_THREADS; o <<= 1) {
+        SplFwdO fv = spl_fwdo_identity(); SplBwdO gv = spl_bwdo_identity();
+        if (tid >= o) fv = sf[tid - o];
+        if (tid + o < SP_THREADS) gv = sb[tid + o];
+        __syncthreads();
+        sf[tid] = spl_fwdo_combine(fv, sf[tid]); sb[tid] = spl_bwdo_combine(sb[tid], gv);
+        __syncthreads();
+    }
+    SplFwdO frun = fpart[blockIdx.x];
+    if (tid > 0) frun = spl_fwdo_combine(frun, sf[tid - 1]);
+    SplBwdO grun = bpart[blockIdx.x];
+    if (tid + 1 < SP_THREADS) grun = spl_bwdo_combine(sb[tid + 1], grun);
+    SplBwdO gi[SP_ITEMS];
+#pragma unroll
+    for (int k = SP_ITEMS - 1; k >= 0; --k) { grun = spl_bwdo_combine(ge[k], grun); gi[k] = grun; }
+    u32 out[SP_ITEMS];
+#pragma unroll
+    for (int k = 0; k < SP_ITEMS; ++k) {
+        const u64 i = base + k;
+        const u32 state = spl_fwdo_state(frun);   // the automaton's state before byte i
+        frun = spl_fwdo_combine(frun, fe[k]);
+        const bool st = i < n && (mm[k] & SM_START) && spl_chunk_start_o200k<WITH_B>(i, n, state, gi[k], B, M, contr);
+        out[k] = TOKENS ? ((u32)s_b[SP_HALO + tid * SP_ITEMS + k] | (st ? TOK_FLAG : 0u)) : (st ? 1u : 0u);
+    }
+    if (TOKENS) {
+        if (base + SP_ITEMS <= n) {
+            uint4 *d = reinterpret_cast<uint4 *>(dst + base);
+            d[0] = make_uint4(out[0], out[1], out[2], out[3]);
+            d[1] = make_uint4(out[4], out[5], out[6], out[7]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) dst[base + k] = out[k];
+        }
+    } else {
+        if (base + SP_ITEMS <= n) {
+            *reinterpret_cast<uint2 *>(flag + base) = make_uint2(out[0] | (out[1] << 8) | (out[2] << 16) | (out[3] << 24),
+                                                                 out[4] | (out[5] << 8) | (out[6] << 16) | (out[7] << 24));
+        } else {
+#pragma unroll
+            for (int k = 0; k < SP_ITEMS; ++k) if (base + k < n) flag[base + k] = (unsigned char)out[k];
+        }
+    }
+}
+
 // per tile: scans + rule.  TOKENS = false: flag[i] = 1 at chunk starts.  TOKENS = true: dst[i] = byte | chunk mark.
-// PATTERN: 0 = the GPT-4 split pattern, 1 = the GPT-2 one (split_logic.h: same scans, another rule).
+// PATTERN: 0 = the GPT-4 split pattern, 1 = the GPT-2 one (split_logic.h: same scans, another rule), 3 = the o200k one
+// (split_apply_o200k above; fpart / bpart then hold the SplFwdO / SplBwdO prefixes of k_split_reduce<WITH_B, 3>).
 template <bool TOKENS, bool WITH_B, int PATTERN>
 __global__ void __launch_bounds__(SP_THREADS) k_split_apply(const unsigned char *__restrict__ b, const unsigned char *__restrict__ meta, u64 n,
                                                             const unsigned char *__restrict__ contr,
                                                             const SplFwd *__restrict__ fpart, const SplBwd *__restrict__ bpart,
                                                             unsigned char *__restrict__ flag, u32 *__restrict__ dst) {
+    if constexpr (PATTERN == 3) {
+        split_apply_o200k<TOKENS, WITH_B>(b, meta, n, contr, reinterpret_cast<const SplFwdO *>(fpart), reinterpret_cast<const SplBwdO *>(bpart),
+                                          flag, dst);
+        return;
+    }
     __shared__ __align__(16) unsigned char s_b[SP_TILE + 2 * SP_HALO];
     __shared__ __align__(16) unsigned char s_m[SP_TILE + 2 * SP_HALO];
     __shared__ SplFwd sf[SP_THREADS];

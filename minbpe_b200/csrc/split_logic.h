@@ -251,3 +251,177 @@ SPL_HD bool spl_chunk_start_gpt2(uint64_t i, uint64_t n, SplFwd f, SplBwd g, con
     }
     return false;
 }
+
+// ---- the o200k pattern (GPT-4o, tiktoken o200k_base) on scans of its own --------------------------------------------
+//   [^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]*[\p{Ll}\p{Lm}\p{Lo}\p{M}]+(?i:'s|'t|'re|'ve|'m|'ll|'d)?
+//  |[^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]+[\p{Ll}\p{Lm}\p{Lo}\p{M}]*(?i:'s|'t|'re|'ve|'m|'ll|'d)?
+//  |\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n/]*|\s*[\r\n]+|\s+(?!\S)|\s+
+// Derivation: DESIGN.md §17.  Words are runs of "case letters" (Lu/Lt, Ll, Lm/Lo and the marks \p{M}, which are no \p{L});
+// a run is cut at an upper-case letter whose last non-Lm/Lo/M letter in front is lower-case, and at the upper-case tail of a
+// run that has no lower-case letter or Lm/Lo/M after it.  What a character does at the edge of a run depends on how far the
+// matches before it reach (a mark is eaten by " ?[^\s\p{L}\p{N}]+", a '/' or newline by its tail "[\r\n/]*", an apostrophe
+// by a contraction), which no run length bounds.  So the forward scan is a small automaton: its value is the map
+// state-before -> state-after of a stretch of text, and maps compose.  The backward scan is SplBwd's over the o200k runs,
+// plus "every letter from here to the end of the word is upper-case".
+//
+// meta bits 5-7: the case class of the character, from the o200k class table (bpe_o200k_table); 0 = not a case letter
+#define SM_CASE_SHIFT 5u
+#define SM_CASE (7u << SM_CASE_SHIFT)
+#define SC_CU 1u   // \p{Lu} \p{Lt}: upper-case only
+#define SC_CL 2u   // \p{Ll}: lower-case only
+#define SC_CB 3u   // \p{Lm} \p{Lo}: both classes
+#define SC_CM 4u   // \p{M}: both classes, and not \p{L}
+SPL_HD uint32_t spl_case(uint32_t m) { return (m & SM_CASE) >> SM_CASE_SHIFT; }
+// run kind under o200k: case letters (marks included) form one kind; digits, whitespace and the rest as spl_kind
+#define SPL_KIND_WORD 8u
+SPL_HD uint32_t spl_kind_o200k(uint32_t m) { return spl_case(m) ? SPL_KIND_WORD : spl_kind(m & SM_CLS); }
+
+// automaton states: what the match that holds a character does with the next one
+#define SO_X 0u    // nothing carries over: the next character starts from scratch (also: an O character taken as the
+                   // [^\r\n\p{L}\p{N}] prefix of the word that follows, the last letter of a contraction)
+#define SO_OM 1u   // inside " ?[^\s\p{L}\p{N}]+": takes further O characters and marks
+#define SO_TL 2u   // inside its tail [\r\n/]*
+#define SO_WN 3u   // inside a word; no Lu/Lt/Ll letter yet (only Lm/Lo/M)
+#define SO_WU 4u   // inside a word; the last letter that is not Lm/Lo/M is upper-case
+#define SO_WL 5u   // inside a word; ... lower-case
+#define SO_C1 6u   // inside a contraction, one letter to go
+#define SO_C2 7u   // ... two letters to go
+#define SO_D1 8u   // inside \p{N}{1,3}, one digit taken
+#define SO_D2 9u   // ... two digits taken
+#define SO_NSTATES 10u
+SPL_HD bool spl_o_in_word(uint32_t t) { return t == SO_WN || t == SO_WU || t == SO_WL; }
+
+// forward value: 4 bits per state s = the state after the stretch when entered in state s
+struct SplFwdO {
+    uint64_t map;
+};
+SPL_HD SplFwdO spl_fwdo_identity() {
+    SplFwdO r; r.map = 0;
+    for (uint32_t s = 0; s < SO_NSTATES; ++s) r.map |= (uint64_t)s << (4 * s);
+    return r;
+}
+SPL_HD SplFwdO spl_fwdo_const(uint32_t to) {
+    SplFwdO r; r.map = 0;
+    for (uint32_t s = 0; s < SO_NSTATES; ++s) r.map |= (uint64_t)to << (4 * s);
+    return r;
+}
+SPL_HD void spl_fwdo_set(SplFwdO &f, uint32_t s, uint32_t to) { f.map = (f.map & ~(0xfull << (4 * s))) | ((uint64_t)to << (4 * s)); }
+// the state after the stretch when the text before it left state s (the text starts in SO_X)
+SPL_HD uint32_t spl_fwdo_state(SplFwdO f, uint32_t s = SO_X) { return (uint32_t)(f.map >> (4 * s)) & 0xfu; }
+// a = everything to the left, b = what follows it
+SPL_HD SplFwdO spl_fwdo_combine(SplFwdO a, SplFwdO b) {
+    SplFwdO r; r.map = 0;
+    for (uint32_t s = 0; s < SO_NSTATES; ++s) r.map |= (uint64_t)spl_fwdo_state(b, spl_fwdo_state(a, s)) << (4 * s);
+    return r;
+}
+
+// first byte of the character after the one that starts at byte j (n if none)
+template <class Meta>
+SPL_HD uint64_t spl_next_char(const Meta &meta, uint64_t n, uint64_t j) {
+    uint64_t k = j + 1;
+    while (k < n && k < j + 4 && !(meta(k) & SM_START)) ++k;
+    return k < n ? k : n;
+}
+// contraction after the apostrophe, with its letters inside the same text (WITH_B: no boundary byte among them)
+template <bool WITH_B, class Bytes, class Meta>
+SPL_HD uint32_t spl_contraction_len_o200k(const Bytes &b, const Meta &meta, uint64_t n, const uint8_t *contr, uint64_t s) {
+    if (s >= n || (WITH_B && (meta(s) & SM_CLS) == SC_B)) return 0;
+    const uint32_t clen = spl_contraction_len(b, n, contr, s);
+    if (WITH_B && clen == 3u && (meta(spl_next_char(meta, n, s)) & SM_CLS) == SC_B) return 0;
+    return clen;
+}
+
+// element of byte j: the transition of the character that starts there (identity on its other bytes)
+template <bool WITH_B, class Bytes, class Meta>
+SPL_HD SplFwdO spl_fwdo_elem(uint64_t j, uint64_t n, const Bytes &b, const Meta &meta, const uint8_t *contr) {
+    const uint32_t m = meta(j);
+    if (!(m & SM_START)) return spl_fwdo_identity();
+    const uint32_t cls = m & SM_CLS, cs = spl_case(m);
+    if (WITH_B && cls == SC_B) return spl_fwdo_const(SO_X);        // the next text starts from scratch
+    if (cls == SC_SP) return spl_fwdo_const(SO_X);
+    SplFwdO f;
+    if (cls == SC_N) {
+        f = spl_fwdo_const(SO_D1);
+        spl_fwdo_set(f, SO_D1, SO_D2); spl_fwdo_set(f, SO_D2, SO_X);
+    } else if (cls == SC_NL) {                                       // the tail of an O match takes newlines
+        f = spl_fwdo_const(SO_X);
+        spl_fwdo_set(f, SO_OM, SO_TL); spl_fwdo_set(f, SO_TL, SO_TL);
+    } else if (cs != 0u) {                                           // case letter or mark
+        const uint32_t fresh = cs == SC_CU ? SO_WU : cs == SC_CL ? SO_WL : SO_WN;
+        f = spl_fwdo_const(fresh);
+        if (cs == SC_CM) spl_fwdo_set(f, SO_OM, SO_OM);              // a mark is also [^\s\p{L}\p{N}]
+        spl_fwdo_set(f, SO_C2, SO_C1); spl_fwdo_set(f, SO_C1, SO_X);
+        if (cs == SC_CB || cs == SC_CM) { spl_fwdo_set(f, SO_WU, SO_WU); spl_fwdo_set(f, SO_WL, SO_WL); }   // SO_WN stays
+    } else {                                                         // O, apostrophe, '/'
+        const uint64_t jn = spl_next_char(meta, n, j);
+        const uint32_t start = (jn < n && spl_case(meta(jn)) != 0u) ? SO_X : SO_OM;   // starts a match: word prefix or O match
+        const uint32_t clen = cls == SC_AP ? spl_contraction_len_o200k<WITH_B>(b, meta, n, contr, jn) : 0u;
+        const uint32_t after_word = clen == 3u ? SO_C2 : clen == 2u ? SO_C1 : start;
+        f = spl_fwdo_const(j > 0 && spl_is_space20<WITH_B>(b, meta, j - 1) ? SO_OM : start);   // " ?[^\s\p{L}\p{N}]+" from the space
+        spl_fwdo_set(f, SO_OM, SO_OM);
+        spl_fwdo_set(f, SO_TL, b(j) == 0x2Fu ? SO_TL : start);
+        spl_fwdo_set(f, SO_WN, after_word); spl_fwdo_set(f, SO_WU, after_word); spl_fwdo_set(f, SO_WL, after_word);
+    }
+    return f;
+}
+
+// backward value: SplBwd over the o200k runs, plus allu = every character of the run from this byte on is Lu/Lt
+struct SplBwdO {
+    uint32_t toend;
+    uint32_t bits;   // nlah | atend << 1 | last << 2 | allu << 3
+};
+#define SPL_B_ALLU 8u
+SPL_HD SplBwdO spl_bwdo_identity() { SplBwdO r; r.toend = 0; r.bits = SPL_B_ALLU; return r; }
+// a = what comes first in the text, b = everything to the right of it
+SPL_HD SplBwdO spl_bwdo_combine(SplBwdO a, SplBwdO b) {
+    if (a.bits & SPL_B_LAST) return a;
+    SplBwdO r;
+    r.toend = a.toend + b.toend;
+    r.bits = (b.bits & (SPL_B_ATEND | SPL_B_LAST)) | ((a.bits | b.bits) & SPL_B_NLAH) | (a.bits & b.bits & SPL_B_ALLU);
+    return r;
+}
+template <bool WITH_B = false>
+SPL_HD SplBwdO spl_bwdo_elem(uint64_t i, uint64_t n, uint32_t m, uint32_t mnext) {
+    const uint32_t cls = m & SM_CLS;
+    const bool last = (i + 1 == n) || spl_kind_o200k(mnext) != spl_kind_o200k(m);
+    const bool text_ends = (i + 1 == n) || (WITH_B && (mnext & SM_CLS) == SC_B);
+    SplBwdO r;
+    r.toend = (m & SM_START) ? 1u : 0u;
+    r.bits = (cls == SC_NL ? SPL_B_NLAH : 0u) | (spl_case(m) == SC_CU ? SPL_B_ALLU : 0u);
+    if (last) r.bits |= SPL_B_LAST | (text_ends ? SPL_B_ATEND : 0u);
+    return r;
+}
+
+// Does a chunk start at byte i (the first byte of a character)?  t = the automaton state before i (spl_fwdo_state of the
+// inclusive forward value at byte i-1; anything for i == 0), g = inclusive backward value at byte i.  Reads b() and meta()
+// at most 1 byte before and 9 bytes after i.  WITH_B as for spl_chunk_start.
+template <bool WITH_B = false, class Bytes, class Meta>
+SPL_HD bool spl_chunk_start_o200k(uint64_t i, uint64_t n, uint32_t t, SplBwdO g, const Bytes &b, const Meta &meta,
+                                  const uint8_t *contr) {
+    if (i == 0) return true;
+    const uint32_t m = meta(i), cls = m & SM_CLS, cs = spl_case(m);
+    if (WITH_B && cls == SC_B) return false;
+    const uint32_t mp = meta(i - 1), pcls = mp & SM_CLS, pcs = spl_case(mp);   // every byte of a character has its meta
+    if (cls == SC_N) return t != SO_D1 && t != SO_D2;                // \p{N}{1,3}
+    if (cls == SC_SP || cls == SC_NL) {                              // as spl_chunk_start, with "the tail takes newlines" from t
+        const bool is_nl = cls == SC_NL;
+        const bool in_run = pcls == SC_SP || pcls == SC_NL;
+        const bool is_w2s = (t == SO_OM || t == SO_TL) ? !is_nl : !in_run;
+        const bool nlah = (g.bits & SPL_B_NLAH) != 0, atend = (g.bits & SPL_B_ATEND) != 0;
+        const bool is_w3s = !nlah && ((pcls == SC_NL && t != SO_TL) || is_w2s);
+        return (is_w2s && nlah) || (is_w3s && (atend || g.toend >= 2u)) || (g.toend == 1u && !atend && !is_nl);
+    }
+    if (cs == 0u) {                                                  // O, apostrophe, '/'
+        if (t == SO_OM) return false;
+        if (t == SO_TL) return b(i) != 0x2Fu;
+        if (spl_o_in_word(t)) return !(cls == SC_AP && spl_contraction_len_o200k<WITH_B>(b, meta, n, contr, i + 1) != 0u);
+        return !spl_is_space20<WITH_B>(b, meta, i - 1);
+    }
+    // case letters and marks
+    if (t == SO_OM) return cs != SC_CM;
+    if (t == SO_C1 || t == SO_C2) return false;
+    if (t == SO_TL) return true;
+    if (spl_o_in_word(t))                                            // a case boundary inside the word
+        return cs == SC_CU && (t == SO_WL || ((pcs == SC_CB || pcs == SC_CM) && (g.bits & SPL_B_ALLU)));
+    return !(pcls == SC_SP || (pcs == 0u && (pcls == SC_O || pcls == SC_AP)));   // a [^\r\n\p{L}\p{N}] prefix starts it
+}

@@ -41,7 +41,7 @@ def shard_chunks(n_bytes, offsets, rank, world):
 
 def first_safe_cut(window):
     """Smallest p >= 1 with window[p-1] an ASCII letter and window[p] == U+0020, or -1.  Such a point is a chunk
-    boundary of the GPT-2/GPT-4 split patterns whatever surrounds it (SURVEY.md §8e): no alternative matches a
+    boundary of the GPT-2/GPT-4/o200k split patterns whatever surrounds it (SURVEY.md §8e, DESIGN.md §17): no alternative matches a
     letter followed by a space inside one chunk, and the patterns have no look-behind, so
     findall(left) + findall(right) == findall(whole)."""
     w = np.asarray(window, dtype=np.uint8)

@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
 OPT_DEDUP_LOG2 = 11
@@ -76,6 +76,7 @@ def load_library():
         "bpe_set_option": ([vp, ci, i64], ci),
         "bpe_debug_table": ([vp, vp, vp, u64, P(u64)], ci),
         "bpe_gpt4_tables": ([vp, vp, vp], ci),
+        "bpe_o200k_table": ([vp, vp], ci),
         "bpe_split_gpt4": ([vp, vp, u64, vp, u64, P(u64)], ci),
         "bpe_decode": ([vp, vp, u64, vp, u64, vp, vp, ctypes.c_int32, vp, u64, P(u64), P(ctypes.c_int64)], ci),
         "bpe_load_text_gpt4": ([vp, vp, u64, P(u64)], ci),
@@ -371,16 +372,19 @@ class Engine:
             self._check(rc, "bpe_debug_table")
             return {(int(p[0]), int(p[1])): int(c) for p, c in zip(pairs[: n.value], counts[: n.value])}
 
-    # ---- GPT-4 split pattern on the device ----
+    # ---- split patterns on the device (GPT-4, GPT-2, o200k) ----
     def _ensure_gpt4_tables(self):
         if not getattr(self, "_gpt4_ready", False):
             from .unicode_tables import tables
             cls, contr = tables()
             self._check(self._lib.bpe_gpt4_tables(self._h, _ptr(cls), _ptr(contr)), "bpe_gpt4_tables")
+            from .unicode_tables import o200k_table
+            self._check(self._lib.bpe_o200k_table(self._h, _ptr(o200k_table())), "bpe_o200k_table")
             self._gpt4_ready = True
 
     def split_gpt4(self, data):
-        """Chunk start offsets (uint64) of utf-8 `data` under GPT4_SPLIT_PATTERN, computed on the GPU."""
+        """Chunk start offsets (uint64) of utf-8 `data` under the split pattern of OPT_SPLIT_PATTERN (GPT-4 by default),
+        computed on the GPU."""
         self._ensure_gpt4_tables()
         b = _u8(data)
         out = np.empty(max(b.size, 1), dtype=np.uint64)
@@ -390,7 +394,7 @@ class Engine:
         return out[: n.value].copy()
 
     def load_text_gpt4(self, data, count_chunks=False):
-        """Upload utf-8 `data`, split it with GPT4_SPLIT_PATTERN on the GPU and make it the current stream."""
+        """Upload utf-8 `data`, split it on the GPU (OPT_SPLIT_PATTERN, GPT-4 by default) and make it the current stream."""
         self._ensure_gpt4_tables()
         b = _u8(data)
         n = ctypes.c_uint64()

@@ -2,9 +2,9 @@
 Host pre-split for large corpora: the reference's ``regex.findall(pattern, text)`` (regex.py:41)
 run on several host cores and returned as chunk start offsets (bytes) instead of a list of str.
 
-The GPT-2/GPT-4 split patterns can be restarted at any point that lies between a letter and a
-following U+0020: no alternative of either pattern matches a letter followed by a space inside
-one chunk, and the patterns have no look-behind, so findall(left) + findall(right) ==
+The GPT-2/GPT-4/o200k split patterns can be restarted at any point that lies between a letter and a
+following U+0020: no alternative of these patterns matches a letter followed by a space inside
+one chunk (DESIGN.md §17 for o200k), and the patterns have no look-behind, so findall(left) + findall(right) ==
 findall(whole) at such a cut (SURVEY.md §8e; tests/test_host.py::test_parallel_split checks it
 against single-process findall).  For any other pattern the split runs in one process.
 """
@@ -14,7 +14,7 @@ import os
 import numpy as np
 import regex as re
 
-from .tokenizer import GPT2_SPLIT_PATTERN, GPT4_SPLIT_PATTERN
+from .tokenizer import GPT2_SPLIT_PATTERN, GPT4_SPLIT_PATTERN, O200K_SPLIT_PATTERN
 
 
 def host_cores():
@@ -30,7 +30,7 @@ def host_cores():
     return max(1, n)
 
 
-_SAFE_PATTERNS = (GPT2_SPLIT_PATTERN, GPT4_SPLIT_PATTERN)
+_SAFE_PATTERNS = (GPT2_SPLIT_PATTERN, GPT4_SPLIT_PATTERN, O200K_SPLIT_PATTERN)
 _G = {}
 
 

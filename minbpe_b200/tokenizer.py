@@ -13,7 +13,7 @@ so callers and the reference's own tests work unchanged; the loops underneath ar
                           splits, else count_chunks + Engine.load_chunks_weighted; then Engine.train: the distinct
                           chunks with their counts, same merges as the whole text
     train_from_iterator -> Engine.dedup_begin / dedup_add_docs / dedup_finish (every document split on its own and
-                          counted on the device, in batches) for the GPT-2 / GPT-4 patterns, else a host count
+                          counted on the device, in batches) for the GPT-2 / GPT-4 / o200k patterns, else a host count
 
 What stays on the host, as in the reference: the regex pre-split for any other pattern and for
 short texts (third-party ``regex`` module, regex.py:41,114), special-token splitting
@@ -34,6 +34,16 @@ from .engine import Engine
 # tiktoken's split patterns, quoted by the reference at regex.py:18-19
 GPT2_SPLIT_PATTERN = r"""'(?:[sdmt]|ll|ve|re)| ?\p{L}+| ?\p{N}+| ?[^\s\p{L}\p{N}]+|\s+(?!\S)|\s+"""
 GPT4_SPLIT_PATTERN = r"""'(?i:[sdmt]|ll|ve|re)|[^\r\n\p{L}\p{N}]?+\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]++[\r\n]*|\s*[\r\n]|\s+(?!\S)|\s+"""
+# tiktoken's o200k pattern (o200k_base / o200k_harmony, GPT-4o), quoted literally
+O200K_SPLIT_PATTERN = "|".join([
+    r"""[^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]*[\p{Ll}\p{Lm}\p{Lo}\p{M}]+(?i:'s|'t|'re|'ve|'m|'ll|'d)?""",
+    r"""[^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]+[\p{Ll}\p{Lm}\p{Lo}\p{M}]*(?i:'s|'t|'re|'ve|'m|'ll|'d)?""",
+    r"""\p{N}{1,3}""",
+    r""" ?[^\s\p{L}\p{N}]+[\r\n/]*""",
+    r"""\s*[\r\n]+""",
+    r"""\s+(?!\S)""",
+    r"""\s+""",
+])
 
 _shared_engine = None
 
@@ -343,14 +353,15 @@ class RegexTokenizer(Tokenizer):
         self.special_tokens = {}
         self.inverse_special_tokens = {}
 
-    # texts at least this long are split on the GPU when the pattern is the GPT-4 one (same chunks as
-    # regex.findall — tests/test_split_rules.py, tests/test_gpu_split.py); short ones stay on the host
+    # texts at least this long are split on the GPU when the pattern is one of _DEVICE_PATTERNS (same chunks as
+    # regex.findall — tests/test_split_rules.py, tests/test_split_rules_o200k.py, tests/test_gpu_split.py); short ones stay
+    # on the host
     DEVICE_SPLIT_MIN_BYTES = 1 << 16
 
-    _DEVICE_PATTERNS = {GPT4_SPLIT_PATTERN: 0, GPT2_SPLIT_PATTERN: 1}     # BPE_OPT_SPLIT_PATTERN values
+    _DEVICE_PATTERNS = {GPT4_SPLIT_PATTERN: 0, GPT2_SPLIT_PATTERN: 1, O200K_SPLIT_PATTERN: 3}   # BPE_OPT_SPLIT_PATTERN values
 
     def _device_split(self, nbytes):
-        """Large texts under one of the reference's two patterns (regex.py:18-19) are split on the GPU; the engine may be
+        """Large texts under one of the reference's two patterns (regex.py:18-19) or the o200k one are split on the GPU; the engine may be
         shared by tokenizers with different patterns, so the pattern is selected before every such call."""
         # the pattern that is actually used for splitting is compiled_pattern (regex.py:32,41,114), not the
         # `pattern` string, which load() may have replaced
@@ -371,7 +382,7 @@ class RegexTokenizer(Tokenizer):
     def train(self, text, vocab_size, verbose=False, *, resume=False, dedup=False):
         """regex.py:35-70.  dedup=True (not in the reference): train on the distinct chunks of the text with their counts,
         which gives the same merges, vocab and verbose lines as dedup=False with less work per merge when chunks
-        repeat, as they do in natural text.  Texts the device splits (GPT-2 / GPT-4 patterns, at least 64 KiB) are
+        repeat, as they do in natural text.  Texts the device splits (GPT-2 / GPT-4 / o200k patterns, at least 64 KiB) are
         split and counted on the device (bpe_load_text_gpt4_dedup); other patterns and short texts are split with
         `regex` and counted on the host (count_chunks)."""
         assert vocab_size >= 256
@@ -394,7 +405,7 @@ class RegexTokenizer(Tokenizer):
         """Train on an iterable of documents (str), not in the reference: the merges, vocab and verbose lines of the
         reference's training loop (regex.py:49-70) on the chunks of every document split on its own, documents in
         iteration order — no chunk spans two documents.  The training runs on the distinct chunks with their counts, as
-        train(dedup=True) does.  For the GPT-2 / GPT-4 patterns the documents are split and counted on the GPU in batches
+        train(dedup=True) does.  For the GPT-2 / GPT-4 / o200k patterns the documents are split and counted on the GPU in batches
         of ITERATOR_BATCH_BYTES (bpe_dedup_add_docs), so the corpus never has to fit in host memory; other patterns are
         split with `regex` and counted on the host.  A non-str item raises TypeError; resume=True as in train()."""
         assert vocab_size >= 256
@@ -433,7 +444,7 @@ class RegexTokenizer(Tokenizer):
         """train() for a UTF-8 text file of any size (not in the reference, which takes a str: regex.py:36).  The file
         is memory-mapped and split on the device in pieces; when torch.distributed is initialised (one process per
         GPU) every rank trains on its own byte range — cut where a letter is followed by a space, a provable chunk
-        boundary of both patterns — and all ranks end with identical merges / vocab.  GPT-2 / GPT-4 split patterns only.
+        boundary of both patterns — and all ranks end with identical merges / vocab.  GPT-2 / GPT-4 / o200k split patterns only.
         dedup=True: train on the file's distinct chunks with their counts, so HBM holds the distinct content rather than
         the file.  On one GPU it counts them there (bpe_load_text_gpt4_dedup); with a process group of more than one rank
         every rank counts its own byte range, the ranks exchange their entries once and every rank merges them and trains
@@ -442,7 +453,7 @@ class RegexTokenizer(Tokenizer):
         assert vocab_size >= 256
         which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
         if which is None:
-            raise ValueError("train_from_file splits on the device and supports the GPT-2 / GPT-4 split patterns only; "
+            raise ValueError("train_from_file splits on the device and supports the GPT-2 / GPT-4 / o200k split patterns only; "
                              "use train(open(path).read(), ...) for other patterns")
         from .engine import OPT_SPLIT_PATTERN
         if dedup:
@@ -479,11 +490,11 @@ class RegexTokenizer(Tokenizer):
     def encode_file(self, path, allowed_special="none", *, group=None, gather=False):
         """encode() for a UTF-8 text file of any size (not in the reference, which takes a str: regex.py:123): the file is
         memory-mapped; with torch.distributed initialised every rank encodes its own byte range and returns its own ids
-        (rank order = text order; gather=True concatenates them on rank 0).  GPT-2 / GPT-4 split patterns, special tokens
+        (rank order = text order; gather=True concatenates them on rank 0).  GPT-2 / GPT-4 / o200k split patterns, special tokens
         within the limits of the device front end.  "none_raise" is not offered: it would scan the file on the host."""
         which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
         if which is None:
-            raise ValueError("encode_file splits on the device and supports the GPT-2 / GPT-4 split patterns only")
+            raise ValueError("encode_file splits on the device and supports the GPT-2 / GPT-4 / o200k split patterns only")
         if allowed_special == "all":
             special = self.special_tokens
         elif allowed_special == "none":
@@ -578,7 +589,7 @@ class RegexTokenizer(Tokenizer):
 
     def encode_batch(self, texts, allowed_special="none_raise"):
         """[self.encode(t, allowed_special) for t in texts], errors included, not in the reference (tiktoken and HF
-        `tokenizers` have it).  For the GPT-2 / GPT-4 patterns and batches of at least DEVICE_SPLIT_MIN_BYTES the documents
+        `tokenizers` have it).  For the GPT-2 / GPT-4 / o200k patterns and batches of at least DEVICE_SPLIT_MIN_BYTES the documents
         go to the GPU in batches of ITERATOR_BATCH_BYTES (bpe_encode_docs): every document is split on its own there, its
         special tokens found inside it only, and every distinct chunk encoded once through the memo.  Anything else is the
         per-document loop."""
