@@ -107,11 +107,13 @@ __global__ void __launch_bounds__(256) k_seg_filter(Ctl *ctl, const Edge *e0, co
 }
 
 // after the merge: the listed segments are the only ones whose tokens can have changed — their signatures from their
-// tokens again (one warp per list entry).  The list is empty when the filter did not run this iteration.
+// tokens again (one warp per list entry).  The list is empty when the filter did not run this iteration (done, a table
+// overflow of an earlier iteration, a pair (a,a)), so a non-empty list is the whole gate of the statistics as well: a
+// merge whose own table update overflowed was performed and counts.
 __global__ void __launch_bounds__(256) k_sig_rebuild_cand(Ctl *ctl, const u32 *__restrict__ buf0, const u32 *__restrict__ buf1,
                                                           const Edge *e0, const Edge *e1, u32 *__restrict__ sig, const u32 *__restrict__ cand) {
     const u32 n = ctl->n_cand;
-    if (blockIdx.x == 0 && threadIdx.x == 0 && !ctl->done && !ctl->overflow && ctl->a != ctl->b && n) {
+    if (blockIdx.x == 0 && threadIdx.x == 0 && n) {
         ctl->cand_sum += n; ctl->seg_sum += ctl->nseg;      // statistics: how much of the stream the filtered merges looked at
     }
     if (!n) return;
