@@ -100,6 +100,16 @@ int bpe_dedup_begin(bpe_handle *h);
 int bpe_dedup_add_docs(bpe_handle *h, const uint8_t *bytes, uint64_t n, const uint64_t *doc_offsets, uint64_t n_docs,
                        uint64_t *n_chunks);
 int bpe_dedup_finish(bpe_handle *h, uint64_t *n_chunks, uint64_t *n_entries);
+/* Training with special tokens (regex.py:152-154, as RegexTokenizer.encode(text, allowed_special="all") splits a text,
+ * applied to the text the loop of regex.py:49-70 trains on): installs special tokens in the open counting session
+ * (k == 0 clears them).  The occurrences re.split would report inside every document of the later bpe_dedup_add_docs
+ * calls are left out of the count: they take no table slot, give no entry and do not count in *n_chunks or
+ * bpe_dedup_stats; the text on either side of one is split on its own, and a longer document is cut into pieces away from
+ * them.  A special never matches across two documents.  The specials' utf-8 bytes back to back in dict order,
+ * special_offsets[k + 1], as bpe_encode_text_gpt4_special takes them (at most 64 of 1..48 bytes, BPE_ERR_ARG otherwise,
+ * leaving the session as it was); no ids, nothing is emitted for an occurrence.  The session keeps its own copy: an encode
+ * with other specials on the handle does not change it.  Outside a session BPE_ERR_STATE. */
+int bpe_dedup_set_specials(bpe_handle *h, const uint8_t *special_bytes, const uint32_t *special_offsets, int32_t k);
 /* Entries built elsewhere, merged into one weighted stream on the device: the weighted streams of a text's consecutive
  * parts (e.g. each rank's bpe_load_text_gpt4_dedup of its byte range, read back with bpe_read_chunk_entries), concatenated
  * in text order.  Arguments and validation (and error codes) as bpe_load_chunks_weighted.  Every entry of <= 48 bytes finds

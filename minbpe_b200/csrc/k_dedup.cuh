@@ -10,6 +10,11 @@
 // A slot's first position is final once its piece is counted (later pieces hold larger positions), so every piece is
 // emitted and dropped before the next one is split.  After the last piece k_dd_weights<false> reads every entry's weight:
 // the slot's count, or 1 for an entry without a slot.
+// With special tokens (a counting session's set, DESIGN.md §18) every accepted occurrence is one chunk of the piece, and
+// mark[p] != 0 on the bytes of the occurrences (k_special_meta<false> on a cleared array): k_dd_count<false, true> gives the
+// chunk of an occurrence no slot and no count but the table's guard slot (index mask + 1, never probed, first position ~0),
+// so k_dd_keep never keeps it.  The text position still runs over the occurrences' bytes, so first occurrences and
+// tie-breaks stay those of the text.
 // bpe_load_chunks_weighted_dedup merges entries that are already weighted (the ranks' streams, back to back) the same way,
 // in one pass over one buffer: k_dd_count<true> adds the entry's weight instead of 1, and k_dd_weights<true> gives an entry
 // without a slot its own weight instead of 1.  The weights are the kernels' last parameters, which the <false>
@@ -102,6 +107,26 @@ __global__ void __launch_bounds__(256) k_dd_keep(const u64 *__restrict__ offs, u
     for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < k; j += (u64)gridDim.x * blockDim.x) {
         const u32 s = slot_of[j];
         keep[j] = (s == DD_NONE || T.s[s].first == text_pos + offs[j]) ? 1 : 0;
+    }
+}
+
+// SPEC: chunk j is a special-token occurrence when mark[offs[j]] != 0; its slot is the guard slot T.mask + 1, it adds no
+// count, and *skipped counts it
+template <bool WEIGHTED, bool SPEC>
+__global__ void __launch_bounds__(256) k_dd_count(const unsigned char *__restrict__ text, u64 m, const u64 *__restrict__ offs,
+                                                  u64 k, u64 text_pos, DdTable T, u32 *__restrict__ slot_of,
+                                                  const u64 *__restrict__ w, const unsigned char *__restrict__ mark,
+                                                  ull *__restrict__ skipped) {
+    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < k; j += (u64)gridDim.x * blockDim.x) {
+        const u64 start = offs[j], end = j + 1 < k ? offs[j + 1] : m;
+        const u64 len = end - start;
+        const ull add = WEIGHTED ? (ull)w[j] : 1ull;
+        if (SPEC && mark[start]) {
+            slot_of[j] = (u32)(T.mask + 1);
+            atomicAdd(skipped, 1ull);
+            continue;
+        }
+        slot_of[j] = len <= DD_KEY_MAX ? dd_count_one(text + start, (u32)len, T, add, text_pos, start) : DD_NONE;
     }
 }
 

@@ -53,24 +53,48 @@ def first_safe_cut(window):
     return int(hit[0]) + 1 if hit.size else -1
 
 
-def shard_byte_range(n_bytes, rank, world, fetch, window=1 << 20, empty_tail=False):
+def shard_byte_range(n_bytes, rank, world, fetch, window=1 << 20, empty_tail=False, specials=None):
     """Byte range [lo, hi) of rank `rank`: the r-th of `world` equal parts of the text, both ends moved forward to
     the next provable chunk boundary (first_safe_cut).  fetch(lo, hi) returns the text bytes [lo, hi) as uint8
     (a slice of an mmap, a generated block, ...).  Rank order = text order.  empty_tail=True: a cut with no boundary
     between it and the end of the text moves to the end of the text (the end is a boundary too), so the ranks after it get
-    empty ranges instead of a ValueError; for callers that handle an empty range (count_file_shard)."""
+    empty ranges instead of a ValueError; for callers that handle an empty range (count_file_shard).  specials: [utf-8
+    bytes, ...] of special tokens; a cut never falls strictly inside an occurrence of one, so every rank sees the
+    occurrences re.split reports in the whole text."""
+    toks = [bytes(t) for t in specials or ()]
+    back = max((len(t) for t in toks), default=0)       # an occurrence that covers a cut starts less than this before it
+
+    def inside_special(raw, p):
+        """does the cut between bytes p-1 and p fall strictly inside an occurrence of a special token?"""
+        return any(raw[p - j: p - j + len(t)] == t for t in toks for j in range(1, len(t)) if p - j >= 0)
+
+    def safe(window_bytes, base):
+        """first letter+space cut at or after window_bytes[base] that does not lie inside an occurrence of a special token,
+        or -1"""
+        w = np.asarray(window_bytes, dtype=np.uint8)
+        raw = w.tobytes()
+        while True:
+            p = first_safe_cut(w[base:])
+            if p < 0:
+                return -1
+            p += base
+            if not inside_special(raw, p):
+                return p
+            base = p
+
     def cut(r):
         if r <= 0:
             return 0
         if r >= world:
             return n_bytes
         lo = n_bytes * r // world
-        p = first_safe_cut(fetch(lo, min(n_bytes, lo + window)))
+        w0 = max(0, lo - back)                          # the window starts early enough to see a special that straddles `lo`
+        p = safe(fetch(w0, min(n_bytes, lo + window)), lo - w0)
         if p < 0 and empty_tail and lo + window >= n_bytes:
             return n_bytes
         if p < 0:
             raise ValueError(f"no letter+space cut point in the {window} bytes after offset {lo}: cannot shard this text")
-        return lo + p
+        return w0 + p
     return cut(rank), cut(rank + 1)
 
 
@@ -278,17 +302,18 @@ def train_file(engine, device, path, num_merges, first_idx=256, group=None, poll
     return tr.result()
 
 
-def count_file_shard(engine, path, rank, world):
+def count_file_shard(engine, path, rank, world, specials=None):
     """The distinct chunks of rank `rank`'s byte range of a text file (shard_byte_range), counted on this rank's GPU
     (Engine.load_text_gpt4_dedup, the engine's split pattern) and read back: -> (entry bytes uint8, entry offsets uint64,
     weights uint64, chunks of the range).  The entries obey DESIGN.md §14's rule for the range; an empty range gives empty
-    arrays.  Needs no process group: a test can play every rank in one process."""
+    arrays.  specials: [utf-8 bytes, ...] of special tokens whose occurrences are left out (DESIGN.md §18); the range
+    never cuts one.  Needs no process group: a test can play every rank in one process."""
     size = os.path.getsize(path)
     mm = np.memmap(path, dtype=np.uint8, mode="r") if size else np.zeros(0, dtype=np.uint8)
-    lo, hi = shard_byte_range(size, rank, world, lambda a, b: mm[a:b], empty_tail=True)
+    lo, hi = shard_byte_range(size, rank, world, lambda a, b: mm[a:b], empty_tail=True, specials=specials)
     if hi <= lo:
         return np.zeros(0, np.uint8), np.zeros(0, np.uint64), np.zeros(0, np.uint64), 0
-    chunks, _ = engine.load_text_gpt4_dedup(mm[lo:hi])
+    chunks, _ = engine.load_text_gpt4_dedup(mm[lo:hi], specials)
     del mm
     data, offsets = engine.chunk_entries()
     return data, offsets, engine.chunk_weights(), int(chunks)
@@ -312,15 +337,15 @@ def _run_digest(pairs, counts, done):
     return int.from_bytes(h.digest()[:8], "little") & ((1 << 63) - 1)
 
 
-def train_file_dedup(engine, path, num_merges, first_idx=256, group=None):
+def train_file_dedup(engine, path, num_merges, first_idx=256, group=None, specials=None):
     """regex.py:36-66 for a text FILE on every rank of a process group, trained on its distinct chunks: every rank counts
     the distinct chunks of its byte range (count_file_shard), the ranks exchange their entries once (one all-gather), every
     rank merges them into the weighted stream of the whole file on its GPU (load_merged_shards) and runs the weighted loop
     there.  No exchange per merge.  Afterwards the ranks compare a 63-bit digest of their merges and counts (all-reduce MIN
-    and MAX) and raise RuntimeError if they differ.  Works over gloo and NCCL groups.  Returns (pairs, counts, n_done),
-    identical on every rank."""
+    and MAX) and raise RuntimeError if they differ.  Works over gloo and NCCL groups.  specials: as count_file_shard.
+    Returns (pairs, counts, n_done), identical on every rank."""
     rank, world = dist.get_rank(group), dist.get_world_size(group)
-    part = count_file_shard(engine, path, rank, world)
+    part = count_file_shard(engine, path, rank, world, specials)
     parts = [None] * world
     dist.all_gather_object(parts, part, group=group)
     load_merged_shards(engine, parts)
@@ -369,39 +394,7 @@ def encode_file(engine, path, merges, byte_perm=None, specials=None, group=None,
             rank, world = 0, 1
     size = os.path.getsize(path)
     mm = np.memmap(path, dtype=np.uint8, mode="r") if size else np.zeros(0, dtype=np.uint8)
-    toks = [t for t, _ in (specials or [])]
-
-    def inside_special(raw, p):
-        """does the cut between bytes p-1 and p fall strictly inside an occurrence of a special token?"""
-        return any(raw[p - j: p - j + len(t)] == t for t in toks for j in range(1, len(t)) if p - j >= 0)
-
-    back = max((len(t) for t in toks), default=0)       # an occurrence that covers a cut starts less than this before it
-
-    def safe(window, base):
-        """first letter+space cut at or after window[base] that does not lie inside an occurrence of a special token, or -1"""
-        w = np.asarray(window, dtype=np.uint8)
-        raw = w.tobytes()
-        while True:
-            p = first_safe_cut(w[base:])
-            if p < 0:
-                return -1
-            p += base
-            if not inside_special(raw, p):
-                return p
-            base = p
-
-    def cut(r):
-        if r <= 0:
-            return 0
-        if r >= world:
-            return size
-        lo = size * r // world
-        w0 = max(0, lo - back)                          # the window starts early enough to see a special that straddles `lo`
-        p = safe(mm[w0: min(size, lo + (1 << 20))], lo - w0)
-        if p < 0:
-            raise ValueError(f"no usable letter+space cut point in the MiB after offset {lo}: cannot shard this text")
-        return w0 + p
-    lo, hi = cut(rank), cut(rank + 1)
+    lo, hi = shard_byte_range(size, rank, world, lambda a, b: mm[a:b], specials=[t for t, _ in (specials or [])])
     ids = engine.encode_text_gpt4(mm[lo:hi], merges, byte_perm, specials=specials) if hi > lo else np.zeros(0, np.int32)
     if not gather:
         return ids

@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
 OPT_DEDUP_LOG2 = 11
@@ -57,6 +57,7 @@ def load_library():
         "bpe_load_text_gpt4_dedup": ([vp, vp, u64, P(u64), P(u64)], ci),
         "bpe_dedup_begin": ([vp], ci),
         "bpe_dedup_add_docs": ([vp, vp, u64, vp, u64, P(u64)], ci),
+        "bpe_dedup_set_specials": ([vp, vp, vp, i32], ci),
         "bpe_dedup_finish": ([vp, P(u64), P(u64)], ci),
         "bpe_dedup_stats": ([vp, vp], ci),
         "bpe_load_chunks_weighted_dedup": ([vp, vp, u64, vp, u64, vp, P(u64)], ci),
@@ -402,11 +403,18 @@ class Engine:
                                                  ctypes.byref(n) if count_chunks else None), "bpe_load_text_gpt4")
         return n.value if count_chunks else None
 
-    def load_text_gpt4_dedup(self, data):
+    def load_text_gpt4_dedup(self, data, specials=None):
         """Upload utf-8 `data`, split it on the GPU (BPE_OPT_SPLIT_PATTERN), count its distinct chunks there and make the
-        weighted stream of the distinct chunks with their counts the current stream.  -> (chunks of the text, entries)."""
+        weighted stream of the distinct chunks with their counts the current stream.  -> (chunks of the text, entries).
+        specials: [utf-8 bytes, ...] in the order of a special_tokens dict — their occurrences are left out, and the parts
+        between them are split on their own (a counting session of one document with them installed)."""
         self._ensure_gpt4_tables()
         b = _u8(data)
+        if specials:
+            self.dedup_begin()
+            self.dedup_set_specials(specials)
+            self.dedup_add_docs(b, [0])
+            return self.dedup_finish()
         nc, ne = ctypes.c_uint64(), ctypes.c_uint64()
         self._check(self._lib.bpe_load_text_gpt4_dedup(self._h, _ptr(b) if b.size else None, b.size, ctypes.byref(nc),
                                                        ctypes.byref(ne)), "bpe_load_text_gpt4_dedup")
@@ -427,6 +435,13 @@ class Engine:
         self._check(self._lib.bpe_dedup_add_docs(self._h, _ptr(b) if b.size else None, b.size, _ptr(o) if o.size else None,
                                                  o.size, ctypes.byref(n)), "bpe_dedup_add_docs")
         return n.value
+
+    def dedup_set_specials(self, specials):
+        """Install special tokens in the open counting session (bpe_dedup_set_specials): [utf-8 bytes, ...] in the order of
+        a special_tokens dict.  Their occurrences in the documents of later dedup_add_docs calls are left out of the count;
+        an empty list clears them."""
+        blob, offs, _ = self._specials([(t, 0) for t in specials]) if specials else (None, None, None)
+        self._check(self._lib.bpe_dedup_set_specials(self._h, _ptr(blob), _ptr(offs), len(specials)), "bpe_dedup_set_specials")
 
     def dedup_finish(self):
         """End the session and make the weighted stream of all its documents the current stream (bpe_dedup_finish).

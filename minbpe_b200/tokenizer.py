@@ -14,6 +14,8 @@ so callers and the reference's own tests work unchanged; the loops underneath ar
                           chunks with their counts, same merges as the whole text
     train_from_iterator -> Engine.dedup_begin / dedup_add_docs / dedup_finish (every document split on its own and
                           counted on the device, in batches) for the GPT-2 / GPT-4 / o200k patterns, else a host count
+    train*(special_tokens=S) -> the same counting session with the specials installed (bpe_dedup_set_specials): their
+                          occurrences are found on the device and left out of the count (DESIGN.md §18)
 
 What stays on the host, as in the reference: the regex pre-split for any other pattern and for
 short texts (third-party ``regex`` module, regex.py:41,114), special-token splitting
@@ -372,6 +374,32 @@ class RegexTokenizer(Tokenizer):
         self.engine.set_option(OPT_SPLIT_PATTERN, which)
         return True
 
+    @staticmethod
+    def _check_specials(special_tokens, vocab_size):
+        """The special_tokens argument of train / train_from_iterator / train_from_file -> a {str: int} dict in its order,
+        or None for None / {}.  ValueError, before any device or file work, for a key that is not a non-empty str, an id
+        that is not an int in [vocab_size, 2**31), or an id used twice."""
+        if special_tokens is None or (isinstance(special_tokens, dict) and not special_tokens):
+            return None
+        if not isinstance(special_tokens, dict):
+            raise ValueError(f"special_tokens must be a dict {{str: int}}, not {type(special_tokens).__name__}")
+        seen = set()
+        for text, idx in special_tokens.items():
+            if not isinstance(text, str) or not text:
+                raise ValueError(f"special token {text!r} is not a non-empty str")
+            if isinstance(idx, bool) or not isinstance(idx, (int, np.integer)) or not vocab_size <= idx < 2 ** 31:
+                raise ValueError(f"special token {text!r}: id {idx!r} is not an int in [vocab_size={vocab_size}, 2**31)")
+            if int(idx) in seen:
+                raise ValueError(f"special token {text!r}: id {idx} is used by another special token")
+            seen.add(int(idx))
+        return {text: int(idx) for text, idx in special_tokens.items()}
+
+    @staticmethod
+    def _ordinary_parts(text, special):
+        """The parts of `text` between the occurrences of the specials: what encode(text, allowed_special) encodes
+        (regex.py:152-163)."""
+        return re.split("(" + "|".join(re.escape(k) for k in special) + ")", text)[0::2]
+
     def _device_specials(self, special):
         """The device front end takes at most 64 specials of 1..48 utf-8 bytes and non-negative int32 ids; anything else
         keeps the reference's host split (below)."""
@@ -379,14 +407,29 @@ class RegexTokenizer(Tokenizer):
         return (0 < len(special) <= E.SPECIAL_MAX and
                 all(isinstance(k, str) and 0 < len(k.encode("utf-8")) <= E.SPECIAL_MAX_BYTES and 0 <= int(v) < 2 ** 31 for k, v in special.items()))
 
-    def train(self, text, vocab_size, verbose=False, *, resume=False, dedup=False):
+    def train(self, text, vocab_size, verbose=False, *, resume=False, dedup=False, special_tokens=None):
         """regex.py:35-70.  dedup=True (not in the reference): train on the distinct chunks of the text with their counts,
         which gives the same merges, vocab and verbose lines as dedup=False with less work per merge when chunks
         repeat, as they do in natural text.  Texts the device splits (GPT-2 / GPT-4 / o200k patterns, at least 64 KiB) are
         split and counted on the device (bpe_load_text_gpt4_dedup); other patterns and short texts are split with
-        `regex` and counted on the host (count_chunks)."""
+        `regex` and counted on the host (count_chunks).
+        special_tokens (not in the reference): {str: int}, ids in [vocab_size, 2**31).  Training sees only the parts of
+        the text between the specials' occurrences, as encode(text, allowed_special="all") splits it, every part split on
+        its own; the specials are then registered (register_special_tokens) and stay out of vocab.  With specials
+        training always runs on the distinct chunks with their counts, whatever `dedup` says (the same merges, DESIGN.md
+        §14): on the device when the text is split there and the specials fit the device front end (at most 64, 1..48
+        utf-8 bytes each), else on the host.  A failed training leaves merges, vocab and special_tokens as they were."""
         assert vocab_size >= 256
+        special = self._check_specials(special_tokens, vocab_size)
         data = text.encode("utf-8")
+        if special:
+            if self._device_specials(special) and self._device_split(len(data)):
+                spec = [k.encode("utf-8") for k in special]
+                self._run_training(lambda: self.engine.load_text_gpt4_dedup(data, spec), vocab_size, verbose, resume=resume)
+                self.register_special_tokens(special)
+            else:
+                self._train_docs([text], vocab_size, verbose, resume, special, None)
+            return
         if self._device_split(len(data)):
             # regex.py:41-44 on the GPU (k_split.cuh); dedup: the distinct chunks counted there too (k_dedup.cuh)
             self._run_training(lambda: (self.engine.load_text_gpt4_dedup if dedup else self.engine.load_text_gpt4)(data),
@@ -401,28 +444,43 @@ class RegexTokenizer(Tokenizer):
     # train_from_iterator hands the device the documents in batches of at least this many utf-8 bytes
     ITERATOR_BATCH_BYTES = 64 << 20
 
-    def train_from_iterator(self, texts, vocab_size, verbose=False, *, resume=False):
+    def train_from_iterator(self, texts, vocab_size, verbose=False, *, resume=False, special_tokens=None):
         """Train on an iterable of documents (str), not in the reference: the merges, vocab and verbose lines of the
         reference's training loop (regex.py:49-70) on the chunks of every document split on its own, documents in
         iteration order — no chunk spans two documents.  The training runs on the distinct chunks with their counts, as
         train(dedup=True) does.  For the GPT-2 / GPT-4 / o200k patterns the documents are split and counted on the GPU in batches
         of ITERATOR_BATCH_BYTES (bpe_dedup_add_docs), so the corpus never has to fit in host memory; other patterns are
-        split with `regex` and counted on the host.  A non-str item raises TypeError; resume=True as in train()."""
+        split with `regex` and counted on the host.  A non-str item raises TypeError; resume=True as in train().
+        special_tokens: as in train(), for every document on its own (a special never matches across two documents); the
+        device counts them when the specials fit its front end, else the host does."""
         assert vocab_size >= 256
-        which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
+        special = self._check_specials(special_tokens, vocab_size)
+        self._train_docs(texts, vocab_size, verbose, resume, special, self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern))
+
+    def _train_docs(self, texts, vocab_size, verbose, resume, special, which):
+        """train_from_iterator's work: `which` = BPE_OPT_SPLIT_PATTERN of a device split, None = split and count on the host.
+        special (None or a checked dict): only the parts between their occurrences are counted, and they are registered
+        after a successful training."""
+        if special and not self._device_specials(special):
+            which = None
         if which is None:
             counts = Counter()
             for doc in texts:
                 if not isinstance(doc, str):
                     raise TypeError(f"train_from_iterator takes str documents, got {type(doc).__name__}")
-                _count_into(counts, *split_text(self.compiled_pattern, doc))
+                for part in (self._ordinary_parts(doc, special) if special else (doc,)):
+                    _count_into(counts, *split_text(self.compiled_pattern, part))
             chunks = _counted(counts)
             self._run_training(lambda: self.engine.load_chunks_weighted(*chunks), vocab_size, verbose, resume=resume)
+            if special:
+                self.register_special_tokens(special)
             return
         from .engine import OPT_SPLIT_PATTERN
         eng = self.engine
         eng.set_option(OPT_SPLIT_PATTERN, which)
         eng.dedup_begin()                          # the session records the pattern
+        if special:
+            eng.dedup_set_specials([k.encode("utf-8") for k in special])
         batch, offs, size = [], [], 0
         for doc in texts:
             if not isinstance(doc, str):
@@ -439,8 +497,10 @@ class RegexTokenizer(Tokenizer):
         if batch:
             eng.dedup_add_docs(b"".join(batch), offs)
         self._run_training(eng.dedup_finish, vocab_size, verbose, resume=resume)
+        if special:
+            self.register_special_tokens(special)
 
-    def train_from_file(self, path, vocab_size, verbose=False, *, group=None, dedup=False):
+    def train_from_file(self, path, vocab_size, verbose=False, *, group=None, dedup=False, special_tokens=None):
         """train() for a UTF-8 text file of any size (not in the reference, which takes a str: regex.py:36).  The file
         is memory-mapped and split on the device in pieces; when torch.distributed is initialised (one process per
         GPU) every rank trains on its own byte range — cut where a letter is followed by a space, a provable chunk
@@ -449,14 +509,20 @@ class RegexTokenizer(Tokenizer):
         the file.  On one GPU it counts them there (bpe_load_text_gpt4_dedup); with a process group of more than one rank
         every rank counts its own byte range, the ranks exchange their entries once and every rank merges them and trains
         on its GPU (dist.train_file_dedup).  A group size that cannot be resolved without an initialised process group
-        raises ValueError."""
+        raises ValueError.  special_tokens: as in train(), on the device only (at most 64 specials of 1..48 utf-8 bytes,
+        else ValueError, as encode_file); training then always runs as with dedup=True, and a rank's byte range never cuts
+        an occurrence."""
         assert vocab_size >= 256
+        special = self._check_specials(special_tokens, vocab_size)
         which = self._DEVICE_PATTERNS.get(self.compiled_pattern.pattern)
         if which is None:
             raise ValueError("train_from_file splits on the device and supports the GPT-2 / GPT-4 / o200k split patterns only; "
                              "use train(open(path).read(), ...) for other patterns")
+        if special and not self._device_specials(special):
+            raise ValueError("train_from_file needs special tokens the device front end takes (at most 64, 1..48 utf-8 bytes each)")
+        spec = [k.encode("utf-8") for k in special] if special else None
         from .engine import OPT_SPLIT_PATTERN
-        if dedup:
+        if dedup or special:
             import torch.distributed as dist
             world = 1
             if group is not None or (dist.is_available() and dist.is_initialized()):
@@ -471,14 +537,16 @@ class RegexTokenizer(Tokenizer):
             eng.set_option(OPT_SPLIT_PATTERN, which)
             if world > 1:
                 from .dist import train_file_dedup
-                pairs, counts, done = train_file_dedup(eng, path, vocab_size - 256, group=group)
+                pairs, counts, done = train_file_dedup(eng, path, vocab_size - 256, group=group, specials=spec)
                 self.last_timing = eng.timing()
                 self._adopt(pairs, counts, done, vocab_size - 256, verbose)
-                return
-            def load():   # the mapping is dropped before the merge loop starts
-                data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) else np.zeros(0, dtype=np.uint8)
-                eng.load_text_gpt4_dedup(data)
-            self._run_training(load, vocab_size, verbose)
+            else:
+                def load():   # the mapping is dropped before the merge loop starts
+                    data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) else np.zeros(0, dtype=np.uint8)
+                    eng.load_text_gpt4_dedup(data, spec)
+                self._run_training(load, vocab_size, verbose)
+            if special:
+                self.register_special_tokens(special)
             return
         from .dist import train_file
         eng = self.engine
