@@ -106,7 +106,7 @@ int bpe_dedup_finish(bpe_handle *h, uint64_t *n_chunks, uint64_t *n_entries);
  * calls are left out of the count: they take no table slot, give no entry and do not count in *n_chunks or
  * bpe_dedup_stats; the text on either side of one is split on its own, and a longer document is cut into pieces away from
  * them.  A special never matches across two documents.  The specials' utf-8 bytes back to back in dict order,
- * special_offsets[k + 1], as bpe_encode_text_gpt4_special takes them (at most 64 of 1..48 bytes, BPE_ERR_ARG otherwise,
+ * special_offsets[k + 1], as bpe_encode_text_gpt4_special takes them (at most 65,536 of 1..48 bytes, BPE_ERR_ARG otherwise,
  * leaving the session as it was); no ids, nothing is emitted for an occurrence.  The session keeps its own copy: an encode
  * with other specials on the handle does not change it.  Outside a session BPE_ERR_STATE. */
 int bpe_dedup_set_specials(bpe_handle *h, const uint8_t *special_bytes, const uint32_t *special_offsets, int32_t k);
@@ -204,7 +204,7 @@ int bpe_encode_text_gpt4(bpe_handle *h, const uint8_t *bytes, uint64_t n, const 
  * that matches at a position wins; matches do not overlap), emits special[part] for every special and
  * encode_ordinary(part) for every part in between.  Here the occurrences are found on the device, become boundaries
  * of the GPT-4 split (the text on either side is split on its own) and single-id entries of the encode memo.
- * special_bytes: the specials' utf-8 bytes back to back, in dict order; special_offsets[n_special + 1]; at most 64
+ * special_bytes: the specials' utf-8 bytes back to back, in dict order; special_offsets[n_special + 1]; at most 65,536
  * specials of 1..48 bytes each (BPE_ERR_ARG otherwise: the caller keeps the host split for those). */
 int bpe_encode_text_gpt4_special(bpe_handle *h, const uint8_t *bytes, uint64_t n, const int32_t *merges, int32_t n_merges,
                                  const uint8_t *byte_perm, const uint8_t *special_bytes, const uint32_t *special_offsets,

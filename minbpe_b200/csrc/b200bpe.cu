@@ -28,7 +28,7 @@
 #include "k_weighted.cuh"
 #include "k_dedup.cuh"
 
-#define BPE_ABI_VERSION 7
+#define BPE_ABI_VERSION 8
 
 namespace {   // the owner types stay private to the library: they add no exported symbol
 

@@ -218,7 +218,9 @@ __global__ void __launch_bounds__(E2_THREADS) k_enc_insert(Enc2 E) {
 }
 
 // Special tokens (regex.py:152-163) as memo entries: the occurrence of a special is one chunk (k_special.cuh) whose
-// "encoding" is its single id.  One thread per special, on a freshly cleared table.
+// "encoding" is its single id.  One thread per special, on a freshly cleared table.  A special is placed within E2_PROBES
+// slots of its home slot, as far as the lookups probe; one that is not raises E2_FAIL_OTHER, and the host then encodes
+// with the general path (enc2_reset_memo).
 __global__ void k_enc_seed_specials(Enc2 E, const unsigned char *__restrict__ blob, const u32 *__restrict__ off,
                                     const int *__restrict__ ids, int k) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -233,7 +235,7 @@ __global__ void k_enc_seed_specials(Enc2 E, const unsigned char *__restrict__ bl
     }
     const u64 tag = e2_tag(kw, len);
     u64 slot = (tag >> 1) & E.memo_mask;
-    for (u64 probe = 0; probe <= E.memo_mask; ++probe) {
+    for (int probe = 0; probe < E2_PROBES; ++probe) {
         const u64 old = atomicCAS((ull *)&E.memo[slot].tag, 0ull, (ull)tag);
         if (old == 0) {
             MemoSlot *m = &E.memo[slot];

@@ -61,12 +61,15 @@ def shard_byte_range(n_bytes, rank, world, fetch, window=1 << 20, empty_tail=Fal
     empty ranges instead of a ValueError; for callers that handle an empty range (count_file_shard).  specials: [utf-8
     bytes, ...] of special tokens; a cut never falls strictly inside an occurrence of one, so every rank sees the
     occurrences re.split reports in the whole text."""
-    toks = [bytes(t) for t in specials or ()]
-    back = max((len(t) for t in toks), default=0)       # an occurrence that covers a cut starts less than this before it
+    by_len = {}                                         # length -> the specials of that length
+    for t in specials or ():
+        by_len.setdefault(len(t), set()).add(bytes(t))
+    back = max(by_len, default=0)                       # an occurrence that covers a cut starts less than this before it
 
     def inside_special(raw, p):
-        """does the cut between bytes p-1 and p fall strictly inside an occurrence of a special token?"""
-        return any(raw[p - j: p - j + len(t)] == t for t in toks for j in range(1, len(t)) if p - j >= 0)
+        """does the cut between bytes p-1 and p fall strictly inside an occurrence of a special token?  One set lookup per
+        (length, start), whatever the number of specials."""
+        return any(raw[p - j: p - j + n] in toks for n, toks in by_len.items() for j in range(1, n) if p - j >= 0)
 
     def safe(window_bytes, base):
         """first letter+space cut at or after window_bytes[base] that does not lie inside an occurrence of a special token,

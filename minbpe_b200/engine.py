@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BPE_LIB_PATH") or os.path.join(_HERE, "csrc", "libb200bpe.so")  # override: A/B builds
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 OPT_KERNEL_TIMING, OPT_RESCAN, OPT_BATCH, OPT_TABLE_LOG2, OPT_SPLIT_PIECE, OPT_VOCAB_CAP, OPT_ENC_MEMO_LOG2, OPT_SPLIT_PATTERN, OPT_HIST_KERNEL, OPT_SEG_FILTER = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10
 OPT_DEDUP_LOG2 = 11
@@ -292,7 +292,7 @@ class Engine:
             return out[: n.value].tobytes(), -1
         raise EngineError("bpe_decode: capacity retry failed")
 
-    SPECIAL_MAX, SPECIAL_MAX_BYTES = 64, 48      # limits of bpe_encode_text_gpt4_special
+    SPECIAL_MAX, SPECIAL_MAX_BYTES = 65536, 48   # limits of bpe_encode_text_gpt4_special
 
     def encode_text_gpt4(self, data, merges, byte_perm=None, out=None, specials=None):
         """-> ids int32 of utf-8 `data`: GPT-4 split + encode, both on the GPU (regex.py:111-121).

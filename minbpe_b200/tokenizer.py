@@ -401,7 +401,7 @@ class RegexTokenizer(Tokenizer):
         return re.split("(" + "|".join(re.escape(k) for k in special) + ")", text)[0::2]
 
     def _device_specials(self, special):
-        """The device front end takes at most 64 specials of 1..48 utf-8 bytes and non-negative int32 ids; anything else
+        """The device front end takes at most 65,536 specials of 1..48 utf-8 bytes and non-negative int32 ids; anything else
         keeps the reference's host split (below)."""
         E = Engine
         return (0 < len(special) <= E.SPECIAL_MAX and
@@ -417,8 +417,8 @@ class RegexTokenizer(Tokenizer):
         the text between the specials' occurrences, as encode(text, allowed_special="all") splits it, every part split on
         its own; the specials are then registered (register_special_tokens) and stay out of vocab.  With specials
         training always runs on the distinct chunks with their counts, whatever `dedup` says (the same merges, DESIGN.md
-        §14): on the device when the text is split there and the specials fit the device front end (at most 64, 1..48
-        utf-8 bytes each), else on the host.  A failed training leaves merges, vocab and special_tokens as they were."""
+        §14): on the device when the text is split there and the specials fit the device front end (at most 65,536,
+        1..48 utf-8 bytes each), else on the host.  A failed training leaves merges, vocab and special_tokens as they were."""
         assert vocab_size >= 256
         special = self._check_specials(special_tokens, vocab_size)
         data = text.encode("utf-8")
@@ -509,7 +509,7 @@ class RegexTokenizer(Tokenizer):
         the file.  On one GPU it counts them there (bpe_load_text_gpt4_dedup); with a process group of more than one rank
         every rank counts its own byte range, the ranks exchange their entries once and every rank merges them and trains
         on its GPU (dist.train_file_dedup).  A group size that cannot be resolved without an initialised process group
-        raises ValueError.  special_tokens: as in train(), on the device only (at most 64 specials of 1..48 utf-8 bytes,
+        raises ValueError.  special_tokens: as in train(), on the device only (at most 65,536 specials of 1..48 utf-8 bytes,
         else ValueError, as encode_file); training then always runs as with dedup=True, and a rank's byte range never cuts
         an occurrence."""
         assert vocab_size >= 256
@@ -519,7 +519,7 @@ class RegexTokenizer(Tokenizer):
             raise ValueError("train_from_file splits on the device and supports the GPT-2 / GPT-4 / o200k split patterns only; "
                              "use train(open(path).read(), ...) for other patterns")
         if special and not self._device_specials(special):
-            raise ValueError("train_from_file needs special tokens the device front end takes (at most 64, 1..48 utf-8 bytes each)")
+            raise ValueError("train_from_file needs special tokens the device front end takes (at most 65,536, 1..48 utf-8 bytes each)")
         spec = [k.encode("utf-8") for k in special] if special else None
         from .engine import OPT_SPLIT_PATTERN
         if dedup or special:
@@ -572,7 +572,7 @@ class RegexTokenizer(Tokenizer):
         else:
             raise ValueError(f"allowed_special={allowed_special} not understood (encode_file takes 'all', 'none' or a set)")
         if special and not self._device_specials(special):
-            raise ValueError("encode_file needs special tokens the device front end takes (at most 64, 1..48 utf-8 bytes each)")
+            raise ValueError("encode_file needs special tokens the device front end takes (at most 65,536, 1..48 utf-8 bytes each)")
         from .dist import encode_file
         from .engine import OPT_SPLIT_PATTERN
         eng = self.engine
