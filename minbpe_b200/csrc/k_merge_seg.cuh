@@ -5,8 +5,8 @@
 //
 //   read   4 * count bytes per segment        (one 1-D bulk async copy, TMA / UBLKCP, into the
 //                                              warp's private mbarrier ring, MS_STAGES deep)
-//   write  only from the first 128-token row that changed to the new end of the segment
-//          (16-byte stores, same address range); nothing for an untouched segment
+//   write  only from the 32-byte sector that holds the segment's first changed token to the new end of the
+//          segment (16-byte stores, same address range); nothing for an untouched segment
 //   + 32-byte edge records per segment (first 3 / last 2 tokens, count), double-buffered, so a
 //     warp can see across its segment boundaries without reading a body that another warp rewrites
 //
@@ -21,7 +21,9 @@
 //
 // Statistics delta per warp: the segment's merge starts go to a per-warp list (warp prefix of the lanes' counts), the
 // warp takes them 32 at a time, one per lane, and equal delta indices are folded across the warp with
-// __match_any_sync, so the CTA's delta cache sees one shared atomic per distinct index and round.
+// __match_any_sync, so the CTA's hashed delta cache sees one shared atomic per distinct index and round.  When the pass's
+// NK·(2V+1) delta indices fit in MS_DELTA_WORDS, every index has its own shared counter instead, and each lane adds to
+// it with one shared reduction.
 #pragma once
 #include "common.cuh"
 #include "k_merge.cuh"
@@ -47,18 +49,26 @@
 #define MS_SW (SEG_TOKENS + 8)              // words per stage: pad, body, three following tokens
 #define MS_META 16                          // per stage: P0 P1 N0 N1 N2 seg count - | the segment's own edge record
 #define MS_BE (MS_BATCH + 2)                // edge records of a batch and of the segment on either side
-#define MS_DCACHE (1 << MS_DCACHE_LOG2)     // slots of the per-CTA delta cache (shared memory)
+#define MS_DCACHE (1 << MS_DCACHE_LOG2)     // slots of the per-CTA hashed delta cache (shared memory)
+#ifndef MS_DELTA_WORDS
+#define MS_DELTA_WORDS 3032                 // shared words per CTA for the delta: direct counters, or the hashed cache
+#endif
 #define MS_LIST (SEG_TOKENS / 2)            // merge starts of a segment: never two adjacent tokens, so at most half of them
 #define MS_WARP_WORDS (MS_STAGES * MS_SW + MS_STAGES * MS_META + MS_BE * 8 + MS_LIST)
-#define MS_SMEM_BYTES (MS_WARPS * MS_WARP_WORDS * 4 + MS_WARPS * MS_STAGES * 8 + MS_DCACHE * 8 + 16)
+#define MS_SMEM_BYTES (MS_WARPS * MS_WARP_WORDS * 4 + MS_WARPS * MS_STAGES * 8 + MS_DELTA_WORDS * 4 + 16)
 #define MS_INVALID 0xffffffffu
 static_assert(SEG_TOKENS == 512, "k_merge_seg: a lane owns 4 rows x 4 tokens of a 512-token segment");
 static_assert((MS_SW * 4) % 16 == 0 && (MS_WARP_WORDS * 4) % 16 == 0, "bulk-copy destinations must stay 16-byte aligned");
+static_assert(MS_DELTA_WORDS >= 2 * MS_DCACHE && MS_DELTA_WORDS % 2 == 0, "the hashed cache lives in the delta words");
+// an H100 SM has 228 KB of shared memory and reserves 1 KB of it per CTA
+static_assert(MS_MINBLOCKS * (MS_SMEM_BYTES + 1024) <= 228 * 1024, "MS_MINBLOCKS CTAs of k_merge_seg must share an SM");
 
-// delta[idx] += cnt through a CTA-private shared-memory cache: the same few neighbour ids are hit by
+// delta[idx] += cnt through CTA-private shared-memory counters: the same few neighbour ids are hit by
 // almost every merge of a dense iteration (global same-address atomics serialise in L2); the
-// persistent CTA folds them here and flushes once at exit.
+// persistent CTA folds them here and flushes once at exit.  s_dkey == NULL: every delta index of the pass has its
+// own counter, s_dcnt[idx]; otherwise the counters are a hashed cache of MS_DCACHE slots.
 __device__ __noinline__ void delta_cache_add(u32 *s_dkey, u32 *s_dcnt, ull *delta, u32 idx, u32 cnt) {
+    if (!s_dkey) { atomicAdd(&s_dcnt[idx], cnt); return; }
     u32 slot = (idx * 2654435761u) >> (32 - MS_DCACHE_LOG2);
 #pragma unroll 1
     for (int probe = 0; probe < 4; ++probe) {
@@ -130,9 +140,14 @@ __device__ __forceinline__ void start_delta(u32 at, const Members<NK> &M, u32 z,
              ? base + (mr == j ? 2u * V : V + (mr < j ? z + mr : tp2)) : MS_INVALID;
 }
 
-// one delta index per lane (MS_INVALID: none), added to the cache once per distinct index: the lowest lane of each
-// group of equal indices adds the group's size
+// one delta index per lane (MS_INVALID: none) added to the CTA's counters.  Direct counters (s_dkey == NULL): every lane
+// adds its own 1 with one shared reduction, no call.  Hashed cache: once per distinct index, the lowest lane of each
+// group of equal indices adds the group's size.
 __device__ __forceinline__ void delta_fold_add(u32 idx, u32 lane, u32 *s_dkey, u32 *s_dcnt, ull *delta) {
+    if (!s_dkey) {
+        if (idx != MS_INVALID) atomicAdd(&s_dcnt[idx], 1u);
+        return;
+    }
     const u32 grp = __match_any_sync(0xffffffffu, idx);
     if (idx != MS_INVALID && lane == (u32)(__ffs(grp) - 1)) delta_cache_add(s_dkey, s_dcnt, delta, idx, (u32)__popc(grp));
 }
@@ -183,14 +198,29 @@ struct SegArgs {
 
 // one row (128 tokens, 4 per lane): merge starts m, kept tokens, replaced tokens written back to t[].
 // Member j of M becomes z + j.  up: in, lane 31's starts of the row before (bit 3: at its last token); out, this row's.
+// first: the lowest index of a token of this lane that is replaced or dropped (MS_INVALID: none yet).
 template <int R, int NK>
 __device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, const Members<NK> &M, u32 z, u32 (&t)[4],
-                                         u32 &mn, u32 &keep, u32 &dirty, u32 &up) {
+                                         u32 &mn, u32 &keep, u32 &first, u32 &up) {
     const uint4 q = lds128o<R * 512>(la);
     const u32 nx = lds32o<R * 512 + 16>(la);
     t[0] = q.x; t[1] = q.y; t[2] = q.z; t[3] = q.w;
-    const u32 m = (starts(M, t[0], t[1]) ? 1u : 0u) | (starts(M, t[1], t[2]) ? 2u : 0u) | (starts(M, t[2], t[3]) ? 4u : 0u) |
-                  (starts(M, t[3], nx) ? 8u : 0u);
+    u32 jx[4] = {0, 0, 0, 0};   // NK > 1: the member whose left id is id(t[i]), found once by the member test
+    u32 m;
+    if constexpr (NK == 1) {
+        m = (starts(M, t[0], t[1]) ? 1u : 0u) | (starts(M, t[1], t[2]) ? 2u : 0u) | (starts(M, t[2], t[3]) ? 4u : 0u) |
+            (starts(M, t[3], nx) ? 8u : 0u);
+    } else {
+        auto st = [&](u32 x, u32 y, u32 &j) {
+            x &= TOK_MASK;
+            u32 r = TOK_MASK;
+#pragma unroll
+            for (int k = 0; k < NK; ++k) { const bool h = x == M.a[k]; r = h ? M.b[k] : r; j = h ? (u32)k : j; }
+            return y == r;
+        };
+        m = (st(t[0], t[1], jx[0]) ? 1u : 0u) | (st(t[1], t[2], jx[1]) ? 2u : 0u) | (st(t[2], t[3], jx[2]) ? 4u : 0u) |
+            (st(t[3], nx, jx[3]) ? 8u : 0u);
+    }
     // a start at the token in front of this lane's first one: the lane before tested that pair (lane 0: lane 31, row before)
     const u32 pm = __shfl_sync(0xffffffffu, lane == 31 ? up : m, (lane + 31) & 31) >> 3;
     up = m;
@@ -202,18 +232,13 @@ __device__ __forceinline__ void mark_row(u32 la, u32 lane, u32 count, const Memb
     }
     mn = m & valid;                         // a merge only starts at a token this segment owns
     keep = ~d & valid;
-    dirty |= (mn | (keep ^ valid)) ? (1u << R) : 0u;
+    const u32 changed = mn | (keep ^ valid);
+    if (changed && first == MS_INVALID) first = R * 128u + lane * 4u + (u32)(__ffs(changed) - 1);   // rows come in order
     if (mn) {                               // few lanes: the merged token takes its place in the registers
-        auto zof = [&](u32 x) {
-            u32 id = z;
-#pragma unroll
-            for (int j = 1; j < NK; ++j) if ((x & TOK_MASK) == M.a[j]) id = z + j;
-            return id | (x & TOK_FLAG);
-        };
-        if (mn & 1u) t[0] = zof(t[0]);
-        if (mn & 2u) t[1] = zof(t[1]);
-        if (mn & 4u) t[2] = zof(t[2]);
-        if (mn & 8u) t[3] = zof(t[3]);
+        if (mn & 1u) t[0] = (z + jx[0]) | (t[0] & TOK_FLAG);
+        if (mn & 2u) t[1] = (z + jx[1]) | (t[1] & TOK_FLAG);
+        if (mn & 4u) t[2] = (z + jx[2]) | (t[2] & TOK_FLAG);
+        if (mn & 8u) t[3] = (z + jx[3]) | (t[3] & TOK_FLAG);
     }
 }
 
@@ -242,9 +267,8 @@ __device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     u32 *s_warp = reinterpret_cast<u32 *>(smem_raw);                              // [MS_WARPS][MS_WARP_WORDS]
     u64 *s_bar = reinterpret_cast<u64 *>(s_warp + MS_WARPS * MS_WARP_WORDS);      // [MS_WARPS][MS_STAGES]
-    u32 *s_dkey = reinterpret_cast<u32 *>(s_bar + MS_WARPS * MS_STAGES);          // [MS_DCACHE] delta index or 0xffffffff
-    u32 *s_dcnt = s_dkey + MS_DCACHE;                                             // [MS_DCACHE]
-    ull *s_drops = reinterpret_cast<ull *>(s_dcnt + MS_DCACHE);
+    u32 *s_delta = reinterpret_cast<u32 *>(s_bar + MS_WARPS * MS_STAGES);         // [MS_DELTA_WORDS]
+    ull *s_drops = reinterpret_cast<ull *>(s_delta + MS_DELTA_WORDS);
 
     const u32 FULL = 0xffffffffu;
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -261,6 +285,10 @@ __device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
         M.b[j] = j ? (u32)ctl->bat_b[j] : (u32)ctl->b;
     }
     ull *const delta = A.xbase ? x_local_delta(A.xbase, A.xstride) : A.delta;
+    // the pass's NK·(2V+1) delta indices: one shared counter each when they fit (s_dkey = NULL), else the hashed cache
+    const bool direct = (u64)NK * (2ull * A.V + 1) <= MS_DELTA_WORDS;
+    u32 *const s_dkey = direct ? nullptr : s_delta;               // hashed: [MS_DCACHE] delta index or 0xffffffff
+    u32 *const s_dcnt = direct ? s_delta : s_delta + MS_DCACHE;   // [NK·(2V+1)] counters, or the cache's [MS_DCACHE]
     const u32 *__restrict__ cand = LIST ? reinterpret_cast<const u32 *>(ctl->cand_ptr) : nullptr;
     const u32 n_cand = LIST ? ctl->n_cand : 0u;
 
@@ -275,7 +303,10 @@ __device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
         for (int s = 0; s < MS_STAGES; ++s) mbar_init(s_bar + warp * MS_STAGES + s, 1);
         fence_mbar_init();
     }
-    for (u32 i = tid; i < MS_DCACHE; i += MS_THREADS) { s_dkey[i] = 0xffffffffu; s_dcnt[i] = 0; }
+    if (direct)
+        for (u32 i = tid; i < NK * (2u * A.V + 1u); i += MS_THREADS) s_dcnt[i] = 0;
+    else
+        for (u32 i = tid; i < MS_DCACHE; i += MS_THREADS) { s_dkey[i] = 0xffffffffu; s_dcnt[i] = 0; }
     if (tid == 0) *s_drops = 0;
     __syncthreads();
 
@@ -378,20 +409,23 @@ __device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
 
         // ---- mark: row r = tokens [128r, 128r+128), four consecutive tokens per lane ----
         u32 t[4][4], mn[4] = {0, 0, 0, 0}, keep[4] = {0, 0, 0, 0};
-        u32 dirty = 0;
+        u32 first = MS_INVALID;
         const u32 la = s_a + lane * 16;
         u32 up = starts(M, lds32o<-4>(s_a), lds32(s_a)) ? 8u : 0u;   // the pair (s[-1], s[0]), as lane 31 of row -1
-        mark_row<0>(la, lane, count, M, z, t[0], mn[0], keep[0], dirty, up);
-        if (count > 128u) mark_row<1>(la, lane, count, M, z, t[1], mn[1], keep[1], dirty, up);
-        if (count > 256u) mark_row<2>(la, lane, count, M, z, t[2], mn[2], keep[2], dirty, up);
-        if (count > 384u) mark_row<3>(la, lane, count, M, z, t[3], mn[3], keep[3], dirty, up);
-        dirty = __reduce_or_sync(FULL, dirty);   // rows in which some token is replaced or dropped
-        if (!dirty) {
+        mark_row<0>(la, lane, count, M, z, t[0], mn[0], keep[0], first, up);
+        if (count > 128u) mark_row<1>(la, lane, count, M, z, t[1], mn[1], keep[1], first, up);
+        if (count > 256u) mark_row<2>(la, lane, count, M, z, t[2], mn[2], keep[2], first, up);
+        if (count > 384u) mark_row<3>(la, lane, count, M, z, t[3], mn[3], keep[3], first, up);
+        // the segment's first replaced or dropped token: the lowest lane whose first change lies in the lowest such row
+        const u32 rows = __reduce_or_sync(FULL, first == MS_INVALID ? 0u : 1u << (first >> 7));
+        if (!rows) {
             // untouched segment: nothing to write, the edge record carries over
             if (lane < 8) reinterpret_cast<u32 *>(&e_next[seg])[lane] = lds32(meta_a + 32 + lane * 4);
             __syncwarp();
             continue;
         }
+
+        first = __shfl_sync(FULL, first, __ffs(__ballot_sync(FULL, (first >> 7) == (u32)(__ffs(rows) - 1))) - 1);
 
         // ---- statistics delta of this segment's merge starts (reads the stage before it is rewritten) ----
         if (delta)
@@ -410,24 +444,25 @@ __device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
         const u32 k0 = tot & 0xffu, k1 = (tot >> 8) & 0xffu, k2 = (tot >> 16) & 0xffu, k3 = tot >> 24;
         const u32 off1 = k0, off2 = k0 + k1, off3 = off2 + k2;
         const u32 new_count = off3 + k3;
-        const int first_dirty = __ffs(dirty) - 1;   // rows in front of it stay where they are
+        const u32 first_dirty = first >> 7;        // rows in front of it stay where they are
         __syncwarp();                               // all lanes hold their tokens; delta reads are done
 
         // ---- compact in place inside the stage, from the first dirty row on ----
-        if (first_dirty <= 0) scatter_row(s_a, lane, 0u, k0, excl & 0xffu, keep[0], t[0]);
+        if (first_dirty == 0) scatter_row(s_a, lane, 0u, k0, excl & 0xffu, keep[0], t[0]);
         if (first_dirty <= 1 && count > 128u) scatter_row(s_a, lane, off1, k1, (excl >> 8) & 0xffu, keep[1], t[1]);
         if (first_dirty <= 2 && count > 256u) scatter_row(s_a, lane, off2, k2, (excl >> 16) & 0xffu, keep[2], t[2]);
         if (count > 384u) scatter_row(s_a, lane, off3, k3, excl >> 24, keep[3], t[3]);
         __syncwarp();
-        // ---- copy-out: 16-byte vectors from the first dirty row to the new end (the up to three
-        //      words past new_count land in the dead part of the segment) ----
+        // ---- copy-out: 16-byte vectors from the 32-byte sector of the first changed token (segments are 2 KB aligned,
+        //      so the stores cover whole sectors) to the new end (the up to three words past new_count land in the
+        //      dead part of the segment) ----
         {
             uint4 *__restrict__ gp = reinterpret_cast<uint4 *>(w + (u64)seg * SEG_TOKENS) + lane;
-            const u32 vend = (new_count + 3u) >> 2;
-            if (first_dirty <= 0 && lane < vend) gp[0] = lds128o<0>(la);
-            if (first_dirty <= 1 && lane + 32u < vend) gp[32] = lds128o<512>(la);
-            if (first_dirty <= 2 && lane + 64u < vend) gp[64] = lds128o<1024>(la);
-            if (lane + 96u < vend) gp[96] = lds128o<1536>(la);
+            const u32 vbeg = (first >> 3) << 1, vend = (new_count + 3u) >> 2;
+            if (lane >= vbeg && lane < vend) gp[0] = lds128o<0>(la);
+            if (lane + 32u >= vbeg && lane + 32u < vend) gp[32] = lds128o<512>(la);
+            if (lane + 64u >= vbeg && lane + 64u < vend) gp[64] = lds128o<1024>(la);
+            if (lane + 96u >= vbeg && lane + 96u < vend) gp[96] = lds128o<1536>(la);
         }
         // ---- the segment's new edge record ----
         {
@@ -446,9 +481,15 @@ __device__ __forceinline__ void merge_seg_pass(const SegArgs &A) {
 
     if (lane == 0 && drops) atomicAdd(s_drops, (ull)drops);
     __syncthreads();
-    if (delta)
-        for (u32 i = tid; i < MS_DCACHE; i += MS_THREADS)
-            if (s_dkey[i] != 0xffffffffu && s_dcnt[i]) atomicAdd(&delta[s_dkey[i]], (ull)s_dcnt[i]);
+    if (delta) {
+        if (direct) {
+            for (u32 i = tid; i < NK * (2u * A.V + 1u); i += MS_THREADS)
+                if (s_dcnt[i]) atomicAdd(&delta[i], (ull)s_dcnt[i]);
+        } else {
+            for (u32 i = tid; i < MS_DCACHE; i += MS_THREADS)
+                if (s_dkey[i] != 0xffffffffu && s_dcnt[i]) atomicAdd(&delta[s_dkey[i]], (ull)s_dcnt[i]);
+        }
+    }
     // ---- exit: the last CTA out publishes the new stream length and flips the edge arrays ----
     if (tid == 0) {
         const ull cta_drops = *s_drops;
