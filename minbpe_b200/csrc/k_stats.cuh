@@ -195,13 +195,19 @@ __global__ void __launch_bounds__(256) k_hist_hash(const u32 *__restrict__ buf0,
     for (u32 t = blockIdx.x * wpb + (threadIdx.x >> 5); t < nseg; t += gridDim.x * wpb) {
         const u32 count = e[t].count;
         const u32 *__restrict__ seg = w + (u64)t * SEG_TOKENS;
-        for (u32 i0 = lane_id() * 4; i0 < count; i0 += 128) {
-            const SegTokens r = seg_load4(seg, count, i0, e, t, nseg);
+        // warp-uniform trip count: every lane reaches every __match_any_sync below, so the full mask names exactly the
+        // lanes that execute it (__activemask() would not guarantee that: lanes past the segment's end leave early)
+        for (u32 base = 0; base < count; base += 128) {
+            const u32 i0 = base + lane_id() * 4;
+            SegTokens r;
+            r.nvalid = 0;
+            if (i0 < count) r = seg_load4(seg, count, i0, e, t, nseg);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const bool valid = ((u32)k < r.nvalid) && !(r.t[k + 1] & TOK_FLAG);
                 const u64 key = valid ? pack_pair(r.t[k] & TOK_MASK, r.t[k + 1]) : KEY_EMPTY;
-                const u32 peers = __match_any_sync(__activemask(), key);
+                __syncwarp();
+                const u32 peers = __match_any_sync(0xffffffffu, key);
                 // the lowest lane of a group also holds the group's smallest position
                 if (valid && (__ffs(peers) - 1) == (int)lane_id()) {
                     const u32 add = __popc(peers);

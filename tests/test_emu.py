@@ -71,6 +71,8 @@ def jobs():
                                     cwd=ROOT, env=_env(lib), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True),
     }
     procs["filter"] = _pytest(lib, [t("test_gpu_zz_filter.py")], order="random", par=3)
+    # the differential fuzz rounds of every training and encode path, under guard pages and races between blocks
+    procs["fuzz_gpu_file"] = _pytest(lib, [t("test_gpu_zz_fuzz.py")], order="random", par=3)
     # __graft_entry__.smoke(): one tiny end-to-end run on cuda:0
     procs["smoke"] = subprocess.Popen([sys.executable, "-c", "import __graft_entry__ as g; g.smoke()"], cwd=ROOT, env=_env(lib),
                                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
@@ -132,6 +134,11 @@ def test_emu_sharded_loop_collective_and_p2p(jobs):
 
 def test_emu_segment_filter_training(jobs):
     out = _finish(jobs, "filter")
+    assert " passed" in out and "failed" not in out
+
+
+def test_emu_differential_fuzz_rounds(jobs):
+    out = _finish(jobs, "fuzz_gpu_file")
     assert " passed" in out and "failed" not in out
 
 
