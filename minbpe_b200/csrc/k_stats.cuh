@@ -8,7 +8,9 @@
 // =============================================================================================
 // Full histograms.  Both walk the segmented stream: one warp per segment (grid-stride), four
 // tokens per thread per step (16-byte loads; segment bases are 2 KB aligned), equal keys inside
-// a warp are folded by __match_any_sync before the global reduction.  Stream position of token i
+// a warp are folded by __match_any_sync before the global reduction.  The fold is sound only because
+// every lane of the warp executes every match: the loop over a segment has a warp-uniform trip count,
+// lanes past the end take part with an empty key, and the mask is the full warp.  Stream position of token i
 // of segment t is t*SEG_TOKENS + i (monotone in stream order, used for first-occurrence order).
 // The pair (last token of t, first token of the next non-empty segment) belongs to segment t.
 // =============================================================================================
@@ -42,7 +44,8 @@ __device__ __forceinline__ SegTokens seg_load4(const u32 *__restrict__ seg, u32 
 // BYTE stream (all ids < 256) -> dense 256x256 vector, dense[p0*256+p1] += count.  Used once per
 // train() for iteration 0; afterwards the table is maintained incrementally by the merge pass.
 // Per-block open-addressing histogram in shared memory (text uses a few thousand of the 65,536
-// byte pairs), equal keys of a warp folded first with __match_any_sync, one flush per block.
+// byte pairs), equal keys of a warp folded first with __match_any_sync (all 32 lanes at every match, see above), one
+// flush per block.
 #define HD_SLOTS 4096
 __global__ void __launch_bounds__(256) k_hist_dense(const u32 *__restrict__ buf0, const u32 *__restrict__ buf1,
                                                     const Ctl *__restrict__ ctl, const Edge *e0, const Edge *e1,
@@ -58,15 +61,21 @@ __global__ void __launch_bounds__(256) k_hist_dense(const u32 *__restrict__ buf0
     for (u32 t = blockIdx.x * wpb + (threadIdx.x >> 5); t < nseg; t += gridDim.x * wpb) {
         const u32 count = e[t].count;
         const u32 *__restrict__ seg = w + (u64)t * SEG_TOKENS;
-        for (u32 i0 = lane_id() * 4; i0 < count; i0 += 128) {
-            const SegTokens r = seg_load4(seg, count, i0, e, t, nseg);
+        // warp-uniform trip count, as in k_hist_hash: lanes past the segment's end take part with the empty key, so the
+        // full mask names exactly the lanes that execute each __match_any_sync
+        for (u32 base = 0; base < count; base += 128) {
+            const u32 i0 = base + lane_id() * 4;
+            SegTokens r;
+            r.nvalid = 0;
+            if (i0 < count) r = seg_load4(seg, count, i0, e, t, nseg);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const u32 left = r.t[k] & TOK_MASK, right = r.t[k + 1];
                 const bool valid = ((u32)k < r.nvalid) && !(right & TOK_FLAG);
                 if (valid && (left > 255u || right > 255u)) *err = 1;
                 const u32 key = valid ? ((left & 255u) << 8 | (right & 255u)) : 0xffffffffu;
-                const u32 peers = __match_any_sync(__activemask(), key);
+                __syncwarp();
+                const u32 peers = __match_any_sync(0xffffffffu, key);
                 if (valid && (__ffs(peers) - 1) == (int)lane_id()) {   // group leader adds the whole group
                     const u32 add = __popc(peers);
                     u32 slot = (key * 2654435761u) >> (32 - 12);

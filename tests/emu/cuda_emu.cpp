@@ -50,7 +50,11 @@ enum { F_RUN, F_WAIT_BAR, F_WAIT_WARP, F_SPIN, F_DONE };
 static const size_t STACK_BYTES = 192 * 1024;
 static const unsigned MAX_THREADS = 1024;
 
-struct WarpSlot { uint32_t gen, arrived; uint64_t val[32]; };
+// one rendezvous of a warp: what its first lane brought (kind, mask, call site), who has arrived, their values
+struct WarpSlot {
+    uint32_t gen, arrived; uint64_t val[32];
+    int kind; uint32_t mask, first; const char *file; int line;
+};
 struct Warp { WarpSlot slot[2]; uint32_t alive; };
 
 struct Fiber {
@@ -75,6 +79,8 @@ struct Sched {
     void *dyn = nullptr; size_t dyn_cap = 0;
     unsigned long long spins = 0;
     bool in_kernel = false;
+    const char *kernel = nullptr;      // name of the running kernel (reports)
+    dim3 bid;                          // the running block
 };
 static thread_local Sched *tl = nullptr;
 
@@ -129,29 +135,66 @@ static inline bool slot_ready(const Sched *s, const Fiber *f) {
     return f->wslot->gen == f->wgen && (f->wslot->arrived & need) == need;
 }
 
-uint64_t collective(int kind, uint32_t mask, uint64_t val, uint32_t arg) {
+static const char *kind_name(int kind) {
+    static const char *const names[] = {"__shfl_sync", "__shfl_up_sync", "__shfl_down_sync", "__shfl_xor_sync", "__ballot_sync", "__all_sync",
+                                        "__any_sync", "__reduce_or_sync", "__reduce_max_sync", "__syncwarp", "__match_any_sync"};
+    return kind >= 0 && kind <= C_MATCH ? names[kind] : "?";
+}
+
+[[noreturn]] static void warp_rule_broken(const char *what, const Sched *s, const Fiber *f, const WarpSlot &sl, int kind, uint32_t mask,
+                                          const char *file, int line) {
+    fprintf(stderr, "emu: warp collective rule broken (%s) in kernel %s, block (%u,%u,%u), warp %u:\n"
+            "  lane %u is at %s(mask 0x%08x) at %s:%d\n"
+            "  lane %u arrived first at %s(mask 0x%08x) at %s:%d\n"
+            "  (every live lane named in a collective's mask executes that same call: same site, same kind, same mask)\n",
+            what, s->kernel ? s->kernel : "?", s->bid.x, s->bid.y, s->bid.z, f->warp, f->lane, kind_name(kind), mask, file, line, sl.first,
+            kind_name(sl.kind), sl.mask, sl.file, sl.line);
+    abort();
+}
+
+[[noreturn]] void activemask_called(const char *file, int line) {
+    const Sched *s = tl;
+    const Fiber *f = s && s->cur ? s->cur : nullptr;
+    fprintf(stderr, "emu: __activemask() called at %s:%d in kernel %s, warp %u, lane %u: the converged set it returns depends on "
+            "scheduling; name the lanes that execute the collective instead\n",
+            file, line, s && s->kernel ? s->kernel : "?", f ? f->warp : 0u, f ? f->lane : 0u);
+    abort();
+}
+
+static const uint64_t POISON = 0xCDCDCDCDCDCDCDCDull;   // what a shuffle reads from a lane that is not taking part (guard fill)
+
+uint64_t collective(int kind, uint32_t mask, uint64_t val, uint32_t arg, const char *file, int line) {
     Sched *s = tl;
     Fiber *f = s->cur;
     Warp &w = s->warps[f->warp];
     const uint32_t k = f->coll_seq++;
     WarpSlot &sl = w.slot[k & 1u];
-    if (sl.gen != k + 1) { sl.gen = k + 1; sl.arrived = 0; }   // first lane of collective number k
+    if (sl.gen != k + 1) {   // first lane of collective number k: what it brought is what the others must bring
+        sl.gen = k + 1; sl.arrived = 0;
+        sl.kind = kind; sl.mask = mask; sl.file = file; sl.line = line; sl.first = f->lane;
+    }
+    if (!((mask >> f->lane) & 1u)) warp_rule_broken("the calling lane is not in its own mask", s, f, sl, kind, mask, file, line);
+    if (sl.kind != kind) warp_rule_broken("two kinds of collective meet", s, f, sl, kind, mask, file, line);
+    if (sl.mask != mask) warp_rule_broken("two masks meet", s, f, sl, kind, mask, file, line);
+    if (sl.line != line || strcmp(sl.file, file) != 0) warp_rule_broken("two call sites meet", s, f, sl, kind, mask, file, line);
     sl.val[f->lane] = val;
     sl.arrived |= 1u << f->lane;
     f->wslot = &sl; f->wmask = mask; f->wgen = k + 1;
     while (!slot_ready(s, f)) { f->state = F_WAIT_WARP; to_main(); }
-    const uint32_t in = sl.arrived & mask;
+    const uint32_t in = sl.arrived & mask;    // the lanes taking part: every live lane of the mask
     const uint32_t lane = f->lane;
+    auto from = [&](uint32_t src) { return (in >> src) & 1u ? sl.val[src] : POISON; };
     switch (kind) {
-        case C_SHFL: { const uint32_t src = arg & 31u; return (in >> src) & 1u ? sl.val[src] : val; }
-        case C_UP: return (lane >= arg && ((in >> (lane - arg)) & 1u)) ? sl.val[lane - arg] : val;
-        case C_DOWN: return (lane + arg < 32 && ((in >> (lane + arg)) & 1u)) ? sl.val[lane + arg] : val;
-        case C_XOR: { const uint32_t src = (lane ^ arg) & 31u; return (in >> src) & 1u ? sl.val[src] : val; }
+        case C_SHFL: return from(arg & 31u);
+        case C_UP: return lane >= arg ? from(lane - arg) : val;          // no source lane: the caller's own value (CUDA)
+        case C_DOWN: return lane + arg < 32 ? from(lane + arg) : val;
+        case C_XOR: return from((lane ^ arg) & 31u);
         case C_BALLOT: { uint32_t b = 0; for (int l = 0; l < 32; ++l) if (((in >> l) & 1u) && sl.val[l]) b |= 1u << l; return b; }
         case C_ALL: { for (int l = 0; l < 32; ++l) if (((in >> l) & 1u) && !sl.val[l]) return 0; return 1; }
         case C_ANY: { for (int l = 0; l < 32; ++l) if (((in >> l) & 1u) && sl.val[l]) return 1; return 0; }
         case C_OR: { uint64_t r = 0; for (int l = 0; l < 32; ++l) if ((in >> l) & 1u) r |= sl.val[l]; return r; }
         case C_MAX: { uint64_t r = 0; for (int l = 0; l < 32; ++l) if (((in >> l) & 1u) && sl.val[l] > r) r = sl.val[l]; return r; }
+        case C_MATCH: { uint32_t g = 0; for (int l = 0; l < 32; ++l) if (((in >> l) & 1u) && sl.val[l] == val) g |= 1u << l; return g; }
         default: return 0;
     }
 }
@@ -173,7 +216,7 @@ static int order_mode() {
 
 static void run_block(Sched *s, const LaunchCfg &cfg, dim3 bid) {
     const unsigned n = cfg.block.x * cfg.block.y * cfg.block.z;
-    s->nthreads = n; s->alive = n; s->bar_gen = 1; s->bar_arrived = 0;
+    s->nthreads = n; s->alive = n; s->bar_gen = 1; s->bar_arrived = 0; s->bid = bid;
     const unsigned nw = (n + 31) / 32;
     for (unsigned w = 0; w < nw; ++w) {
         s->warps[w].slot[0].gen = s->warps[w].slot[1].gen = 0;
@@ -221,8 +264,17 @@ static void run_block(Sched *s, const LaunchCfg &cfg, dim3 bid) {
         }
         if (!progress && !spinning) {
             if (++idle_rounds > 2) {
-                fprintf(stderr, "emu: block (%u,%u,%u) is deadlocked: %u threads alive, none can run "
-                        "(divergent __syncthreads / collective whose lanes never arrive)\n", bid.x, bid.y, bid.z, s->alive);
+                fprintf(stderr, "emu: kernel %s, block (%u,%u,%u) is deadlocked: %u threads alive, none can run "
+                        "(divergent __syncthreads / collective whose lanes never arrive)\n", s->kernel ? s->kernel : "?", bid.x, bid.y, bid.z,
+                        s->alive);
+                for (unsigned t = 0; t < n && t < 1024; ++t) {
+                    const Fiber &f = s->fib[t];
+                    if (f.state == F_WAIT_WARP) {
+                        fprintf(stderr, "  thread %u (warp %u, lane %u) waits in %s(mask 0x%08x) at %s:%d\n", t, f.warp, f.lane,
+                                kind_name(f.wslot->kind), f.wmask, f.wslot->file, f.wslot->line);
+                        break;
+                    }
+                }
                 for (unsigned t = 0; t < n && t < 1024; ++t)
                     if (s->fib[t].state != F_DONE) { fprintf(stderr, "  thread %u state %d\n", t, s->fib[t].state); break; }
                 abort();
@@ -245,6 +297,7 @@ static unsigned par_threads() {
 
 struct ParJob {
     const LaunchCfg *cfg = nullptr;
+    const char *kernel = nullptr;
     const std::function<void()> *body = nullptr;
     std::atomic<unsigned long long> next{0};
     unsigned long long total = 0;
@@ -268,6 +321,7 @@ static void par_run_blocks(Sched *s, ParJob *j) {
         if (posix_memalign(&s->dyn, 1024, s->dyn_cap)) abort();
     }
     s->body = j->body;
+    s->kernel = j->kernel;
     s->in_kernel = true;
     s->spins = 0;
     for (;;) {
@@ -301,14 +355,15 @@ static void par_worker(ParPool *p) {
     }
 }
 
-static void launch_parallel(Sched *s, const LaunchCfg &cfg, const std::function<void()> &body, unsigned long long nblocks, unsigned par) {
+static void launch_parallel(Sched *s, const LaunchCfg &cfg, const char *kernel, const std::function<void()> &body, unsigned long long nblocks,
+                            unsigned par) {
     static thread_local ParPool *pool = nullptr;      // one pool per calling thread (= per emulated GPU); lives as long as the process
     if (!pool) {
         pool = new ParPool();
         for (unsigned i = 1; i < par; ++i) pool->workers.emplace_back(par_worker, pool);
     }
     ParJob job;
-    job.cfg = &cfg; job.body = &body; job.total = nblocks;
+    job.cfg = &cfg; job.kernel = kernel; job.body = &body; job.total = nblocks;
     {
         std::lock_guard<std::mutex> lk(pool->mu);
         pool->job = &job;
@@ -363,8 +418,9 @@ void launch(const LaunchCfg &cfg, const char *kernel, const void *func, const st
     }
     const unsigned long long nblocks = (unsigned long long)cfg.grid.x * cfg.grid.y * cfg.grid.z;
     const unsigned par = par_threads();
-    if (par > 1 && nblocks > 1) { launch_parallel(s, cfg, body, nblocks, par); return; }
+    if (par > 1 && nblocks > 1) { launch_parallel(s, cfg, kernel, body, nblocks, par); return; }
     s->body = &body;
+    s->kernel = kernel;
     s->in_kernel = true;
     s->spins = 0;
     for (unsigned z = 0; z < cfg.grid.z; ++z)

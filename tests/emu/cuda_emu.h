@@ -14,9 +14,16 @@
 // Execution model
 //   * one CUDA thread = one fiber (own stack, cooperative switch in ~20 instructions); the fibers of a block share
 //     the `__shared__` variables (static thread_local: one block runs at a time per OS thread);
-//   * __syncthreads / warp collectives (__shfl*_sync, __ballot_sync, __all_sync, __reduce_*_sync) are rendezvous
-//     points: a fiber waits there until the other threads of the block / the other lanes named in the mask that are
-//     still alive have arrived — divergence, early exits and data-dependent loops between them behave as on a GPU;
+//   * __syncthreads / warp collectives (__syncwarp, __shfl*_sync, __ballot_sync, __all_sync, __any_sync, __reduce_*_sync,
+//     __match_any_sync) are rendezvous points: a fiber waits there until the other threads of the block / the other lanes
+//     named in the mask that are still alive have arrived — divergence, early exits and data-dependent loops between them
+//     behave as on a GPU;
+//   * warp collectives are held to the rule the kernels are written to: every live lane named in a collective's mask
+//     executes that same call — same call site, same kind, same mask — and the calling lane is in its own mask.  The k-th
+//     collective of every lane of a warp is one rendezvous; the first lane there records its site, kind and mask and every
+//     later lane is compared with them.  A mismatch stops the kernel with both sites.  __activemask() stops the kernel:
+//     without lock-step hardware the converged set has no value, and on a GPU it has one that depends on scheduling.  A
+//     shuffle that reads a lane which is not taking part (exited, or outside the mask) gets the 0xCD guard fill;
 //   * the threads of a block run in thread-index order between two synchronisation points, or — EMU_ORDER=reverse | random —
 //     in another order: a kernel whose result depends on that order has a data race;
 //   * blocks of a grid run one after another in blockIdx order (legal: CUDA promises no inter-block progress);
@@ -62,8 +69,10 @@ namespace emu {
 struct ThreadCtx { dim3 tid, bid, bdim, gdim; };
 ThreadCtx *ctx();                 // the fiber that is running on this OS thread
 void sync_threads();              // __syncthreads
-enum { C_SHFL, C_UP, C_DOWN, C_XOR, C_BALLOT, C_ALL, C_ANY, C_OR, C_MAX, C_SYNC };
-uint64_t collective(int kind, uint32_t mask, uint64_t val, uint32_t arg);
+enum { C_SHFL, C_UP, C_DOWN, C_XOR, C_BALLOT, C_ALL, C_ANY, C_OR, C_MAX, C_SYNC, C_MATCH };
+// one warp collective of the running lane; file:line is its call site
+uint64_t collective(int kind, uint32_t mask, uint64_t val, uint32_t arg, const char *file, int line);
+[[noreturn]] void activemask_called(const char *file, int line);
 void spin();                      // called from every polling load: lets the other fibers run, bounds the wait
 void *dyn_smem();                 // base of the block's dynamic shared memory
 long long clock();                // monotonic "SM clock"
@@ -91,26 +100,30 @@ extern "C" void emu_fail_alloc(unsigned long long k);
 #define EMU_LAUNCH(K, CFG, ARGS) emu::launch(emu::LaunchCfg CFG, EMU_STR(EMU_UNPAREN K), reinterpret_cast<const void *>(&(EMU_UNPAREN K)), [&]() { EMU_UNPAREN K ARGS; })
 
 static inline void __syncthreads() { emu::sync_threads(); }
-static inline void __syncwarp(unsigned mask = 0xffffffffu) { emu::collective(emu::C_SYNC, mask, 0, 0); }
+#define EMU_SITE const char *file = __builtin_FILE(), int line = __builtin_LINE()   /* the caller's file:line */
+#define EMU_AT file, line
+static inline void __syncwarp(unsigned mask = 0xffffffffu, EMU_SITE) { emu::collective(emu::C_SYNC, mask, 0, 0, EMU_AT); }
 static inline void __threadfence() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
-static inline unsigned __activemask() { return 0xffffffffu; }   // only used as the mask of __match_any_sync (below)
+// no kernel may use it: the emulator cannot give it a meaning, and a GPU gives it one that depends on scheduling
+static inline unsigned __activemask(EMU_SITE) { emu::activemask_called(EMU_AT); }
 static inline long long clock64() { return emu::clock(); }
 
 template <class T> static inline uint64_t emu_bits(T v) { uint64_t b = 0; memcpy(&b, &v, sizeof(T)); return b; }
 template <class T> static inline T emu_unbits(uint64_t b) { T v; memcpy(&v, &b, sizeof(T)); return v; }
-template <class T> static inline T __shfl_sync(unsigned m, T v, int src) { static_assert(sizeof(T) <= 8, ""); return emu_unbits<T>(emu::collective(emu::C_SHFL, m, emu_bits(v), (uint32_t)src)); }
-template <class T> static inline T __shfl_up_sync(unsigned m, T v, unsigned d) { return emu_unbits<T>(emu::collective(emu::C_UP, m, emu_bits(v), d)); }
-template <class T> static inline T __shfl_down_sync(unsigned m, T v, unsigned d) { return emu_unbits<T>(emu::collective(emu::C_DOWN, m, emu_bits(v), d)); }
-template <class T> static inline T __shfl_xor_sync(unsigned m, T v, int x) { return emu_unbits<T>(emu::collective(emu::C_XOR, m, emu_bits(v), (uint32_t)x)); }
-static inline unsigned __ballot_sync(unsigned m, int pred) { return (unsigned)emu::collective(emu::C_BALLOT, m, pred != 0, 0); }
-static inline int __all_sync(unsigned m, int pred) { return (int)emu::collective(emu::C_ALL, m, pred != 0, 0); }
-static inline int __any_sync(unsigned m, int pred) { return (int)emu::collective(emu::C_ANY, m, pred != 0, 0); }
-static inline unsigned __reduce_or_sync(unsigned m, unsigned v) { return (unsigned)emu::collective(emu::C_OR, m, v, 0); }
-static inline unsigned __reduce_max_sync(unsigned m, unsigned v) { return (unsigned)emu::collective(emu::C_MAX, m, v, 0); }
-// __match_any_sync(__activemask(), key) folds equal keys of the lanes that happen to be converged.  Every grouping —
-// including "each lane alone" — is a correct outcome of that call (the kernels add popc(group) per group), and
-// the converged set is not defined without lock-step hardware: the emulator returns the singleton group.
-template <class T> static inline unsigned __match_any_sync(unsigned, T) { return 1u << (emu::ctx()->tid.x & 31u); }
+template <class T> static inline T __shfl_sync(unsigned m, T v, int src, EMU_SITE) { static_assert(sizeof(T) <= 8, ""); return emu_unbits<T>(emu::collective(emu::C_SHFL, m, emu_bits(v), (uint32_t)src, EMU_AT)); }
+template <class T> static inline T __shfl_up_sync(unsigned m, T v, unsigned d, EMU_SITE) { return emu_unbits<T>(emu::collective(emu::C_UP, m, emu_bits(v), d, EMU_AT)); }
+template <class T> static inline T __shfl_down_sync(unsigned m, T v, unsigned d, EMU_SITE) { return emu_unbits<T>(emu::collective(emu::C_DOWN, m, emu_bits(v), d, EMU_AT)); }
+template <class T> static inline T __shfl_xor_sync(unsigned m, T v, int x, EMU_SITE) { return emu_unbits<T>(emu::collective(emu::C_XOR, m, emu_bits(v), (uint32_t)x, EMU_AT)); }
+static inline unsigned __ballot_sync(unsigned m, int pred, EMU_SITE) { return (unsigned)emu::collective(emu::C_BALLOT, m, pred != 0, 0, EMU_AT); }
+static inline int __all_sync(unsigned m, int pred, EMU_SITE) { return (int)emu::collective(emu::C_ALL, m, pred != 0, 0, EMU_AT); }
+static inline int __any_sync(unsigned m, int pred, EMU_SITE) { return (int)emu::collective(emu::C_ANY, m, pred != 0, 0, EMU_AT); }
+static inline unsigned __reduce_or_sync(unsigned m, unsigned v, EMU_SITE) { return (unsigned)emu::collective(emu::C_OR, m, v, 0, EMU_AT); }
+static inline unsigned __reduce_max_sync(unsigned m, unsigned v, EMU_SITE) { return (unsigned)emu::collective(emu::C_MAX, m, v, 0, EMU_AT); }
+// the lanes of the mask that arrived with a key equal to this lane's (a rendezvous like the others)
+template <class T> static inline unsigned __match_any_sync(unsigned m, T key, EMU_SITE) {
+    static_assert(sizeof(T) <= 8, "");
+    return (unsigned)emu::collective(emu::C_MATCH, m, emu_bits(key), 0, EMU_AT);
+}
 
 // ---- bit tricks ------------------------------------------------------------------------------------------------
 static inline int __ffs(int v) { return __builtin_ffs(v); }
